@@ -1156,7 +1156,7 @@ __global__ void __launch_bounds__(BA_BLOCK) ba_schur_spmv_warp_smem_kernel(const
 // THE ROOFLINE KERNEL, pass 1 of 2: u_o = J_c p - J_p (H_pp + D_p^2)^-1 sum_track J_p^T J_c p per observation.
 // One thread per observation slot; a block holds whole tracks, so the point-block elimination
 // (z_p = sum J_p^T y, w_p = Hinv z_p) is a shared-memory exchange.  u is written in camera-sorted order and
-// reduced per camera-side block by ba_cam_stream_kernel.
+// reduced per camera-side block by ba_cam_stream_loop_kernel.
 template <int DC>
 __global__ void __launch_bounds__(BA_BLOCK) ba_schur_spmv_kernel(const BaDev D, const double* __restrict__ pvec,
                                                                  double* __restrict__ qvec) {
@@ -1219,11 +1219,7 @@ __global__ void __launch_bounds__(BA_BLOCK) ba_schur_spmv_kernel(const BaDev D, 
   }
 }
 
-// Second SpMV pass (streaming): out[block] += sum over the block's observations of J_c^T u, observations in camera
-// order.  A warp owns BA_CS_TILES (template parameter; B200BA_CS_TILES = 1 | 2 | 4, default 2) consecutive 32-observation tiles; all their loads are issued up front (fully
-// coalesced tile lines), the products are accumulated per lane while the tiles stay inside one (camera, pose) run —
-// runs are thousands of observations long — and reduced with shuffles once per run change / at the end: 6 + nv
-// red.adds per warp.  No shared memory, no barrier.
+// Warp-reduces the per-lane sums of one (camera, pose) run and adds them to the run's pose / camera blocks of out.
 template <int DC>
 __device__ __forceinline__ void ba_cam_stream_flush(double* acc, int run, const BaDev& D, double* __restrict__ out, int lane) {
   if (run < 0) return;
@@ -1239,62 +1235,11 @@ __device__ __forceinline__ void ba_cam_stream_flush(double* acc, int run, const 
   if (lane < 6) { if (rd.x >= 0) atomicAdd(&out[rd.x + lane], mine); }
   else if (lane < 6 + rd.z) { if (rd.y >= 0) atomicAdd(&out[rd.y + lane - 6], mine); }
 }
-template <int DC, int BA_CS_TILES>
-__global__ void __launch_bounds__(BA_BLOCK) ba_cam_stream_kernel(const BaDev D, double* __restrict__ out, int respect_done) {
-  if (respect_done && D.ctl->done) return;
-  const int lane = threadIdx.x & 31;
-  const long long tile0 = ((long long)blockIdx.x * (BA_BLOCK / 32) + (threadIdx.x >> 5)) * BA_CS_TILES;
-  const long long ntiles = (D.nobs_c + 31) >> 5;
-  int run[BA_CS_TILES];
-  float j0[BA_CS_TILES][DC], j1[BA_CS_TILES][DC], uf0[BA_CS_TILES], uf1[BA_CS_TILES];
-#pragma unroll
-  for (int t = 0; t < BA_CS_TILES; ++t) {
-    const long long k = (tile0 + t) * 32 + lane;
-    if (tile0 + t < ntiles) {   // warp-uniform; the padded tail of the last tile is allocated (run = -1 there)
-      run[t] = D.c_run[k];
-#pragma unroll
-      for (int c = 0; c < DC; ++c) { j0[t][c] = D.JcC[BA_JC(c, k)]; j1[t][c] = D.JcC[BA_JC(DC + c, k)]; }
-      { const float2 uu = D.u[k]; uf0[t] = uu.x; uf1[t] = uu.y; }
-    } else {
-      run[t] = -1;
-#pragma unroll
-      for (int c = 0; c < DC; ++c) { j0[t][c] = 0.f; j1[t][c] = 0.f; }
-      uf0[t] = 0.f; uf1[t] = 0.f;
-    }
-  }
-  double acc[DC];
-#pragma unroll
-  for (int c = 0; c < DC; ++c) acc[c] = 0.0;
-  int cur = -1;
-#pragma unroll
-  for (int t = 0; t < BA_CS_TILES; ++t) {
-    const int r0 = __shfl_sync(0xffffffffu, run[t], 0);
-    const bool uniform = __all_sync(0xffffffffu, run[t] == r0);
-    if (uniform) {
-      if (r0 != cur) { ba_cam_stream_flush<DC>(acc, cur, D, out, lane); cur = r0; }
-      if (r0 >= 0) {
-#pragma unroll
-        for (int c = 0; c < DC; ++c) acc[c] += (double)j0[t][c] * (double)uf0[t] + (double)j1[t][c] * (double)uf1[t];
-      }
-    } else {  // the tile straddles a run boundary (or is the ragged tail): per-observation adds (rare)
-      ba_cam_stream_flush<DC>(acc, cur, D, out, lane); cur = -1;
-      if (run[t] >= 0) {
-        const int4 rd = D.runs[run[t]];
-#pragma unroll
-        for (int c = 0; c < DC; ++c) {
-          const double v = (double)j0[t][c] * (double)uf0[t] + (double)j1[t][c] * (double)uf1[t];
-          if (c < 6) { if (rd.x >= 0) atomicAdd(&out[rd.x + c], v); }
-          else if (c < 6 + rd.z) { if (rd.y >= 0) atomicAdd(&out[rd.y + c - 6], v); }
-        }
-      }
-    }
-  }
-  ba_cam_stream_flush<DC>(acc, cur, D, out, lane);
-}
-
-// Looped form of the second pass: a warp walks a contiguous range of tiles, the next tile's loads are issued before the
-// current tile is accumulated (register double buffer), and the shuffle reduction happens only when the (camera, pose)
-// run changes or the range ends — instead of once per tile.
+// Second SpMV pass (streaming): out[block] += sum over the block's observations of J_c^T u, observations in camera
+// order.  A warp walks a contiguous range of 32-observation tiles (fully coalesced tile lines); the next tile's loads
+// are issued before the current tile is accumulated (register double buffer).  The products are accumulated per lane
+// while the tiles stay inside one (camera, pose) run — runs are thousands of observations long — and reduced with
+// shuffles only when the run changes or the range ends: 6 + nv red.adds per run a warp touches.  No shared memory, no barrier.
 template <int DC>
 __global__ void __launch_bounds__(BA_BLOCK) ba_cam_stream_loop_kernel(const BaDev D, double* __restrict__ out, int respect_done,
                                                                       int tiles_per_warp) {
@@ -2091,7 +2036,6 @@ struct BaStreamGuard {
   }
 };
 
-static int g_ba_cs_tiles = 0;   // ba_cam_stream: 0 = looped kernel (default), 1 | 2 | 4 = tiles per warp of the one-shot kernel (B200BA_CS_TILES)
 static int g_ba_spmv_smem = 1;  // pass 1 with p staged in shared memory when it fits (B200BA_SPMV_SMEM=0 disables)
 static int g_ba_sms = 0;
 #define BA_SPMV_SMEM_MAX (72 * 1024)
@@ -2118,20 +2062,12 @@ static void ba_launch_spmv(const BaDev& D, cudaStream_t s) {
     ba_giant_finish_kernel<0><<<D.nblocks_giant1 - D.nblocks_giant0, BA_BLOCK, 0, s>>>(D, D.p);
   }
   if (D.nobs_c) {
-    if (g_ba_cs_tiles == 0) {
-      if (!g_ba_sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&g_ba_sms, cudaDevAttrMultiProcessorCount, dev); }
-      const long long ntiles = (D.nobs_c + 31) / 32;
-      const long long warps = (long long)g_ba_sms * 2 * (BA_BLOCK / 32) * 2;   // two waves of two resident CTAs per SM
-      const int tpw = (int)std::max<long long>(4, (ntiles + warps - 1) / warps);
-      const unsigned grid = (unsigned)((ntiles + (long long)tpw * (BA_BLOCK / 32) - 1) / ((long long)tpw * (BA_BLOCK / 32)));
-      ba_cam_stream_loop_kernel<DC><<<grid, BA_BLOCK, 0, s>>>(D, D.q, 1, tpw);
-    } else {
-      const unsigned per = BA_BLOCK * (unsigned)g_ba_cs_tiles;
-      const unsigned grid = (unsigned)((D.nobs_c + per - 1) / per);
-      if (g_ba_cs_tiles == 4) ba_cam_stream_kernel<DC, 4><<<grid, BA_BLOCK, 0, s>>>(D, D.q, 1);
-      else if (g_ba_cs_tiles == 2) ba_cam_stream_kernel<DC, 2><<<grid, BA_BLOCK, 0, s>>>(D, D.q, 1);
-      else ba_cam_stream_kernel<DC, 1><<<grid, BA_BLOCK, 0, s>>>(D, D.q, 1);
-    }
+    if (!g_ba_sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&g_ba_sms, cudaDevAttrMultiProcessorCount, dev); }
+    const long long ntiles = (D.nobs_c + 31) / 32;
+    const long long warps = (long long)g_ba_sms * 2 * (BA_BLOCK / 32) * 2;   // two waves of two resident CTAs per SM
+    const int tpw = (int)std::max<long long>(4, (ntiles + warps - 1) / warps);
+    const unsigned grid = (unsigned)((ntiles + (long long)tpw * (BA_BLOCK / 32) - 1) / ((long long)tpw * (BA_BLOCK / 32)));
+    ba_cam_stream_loop_kernel<DC><<<grid, BA_BLOCK, 0, s>>>(D, D.q, 1, tpw);
   }
 }
 template <int DC>
@@ -3234,7 +3170,6 @@ static int ba_solve_impl(const b200ba_options* o, b200ba_problem* p, b200ba_summ
   if (mid_smem) BA_CUDA(cudaFuncSetAttribute(ba_pcg_mid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
   const size_t mid_staged = (fused_pcg && nc <= BA_PCG_T * BA_MID_EPT && getenv("B200BA_MID_PLAIN") == nullptr) ? (size_t)nc * BA_MID_STAGE_BYTES_PER_ROW : 0;
   if (mid_staged) BA_CUDA(cudaFuncSetAttribute(ba_pcg_mid_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_PCG_T * BA_MID_EPT * BA_MID_STAGE_BYTES_PER_ROW));
-  if (const char* e = getenv("B200BA_CS_TILES")) { const int t = atoi(e); g_ba_cs_tiles = (t == 4 || t == 2 || t == 1) ? t : 0; }
   if (const char* e = getenv("B200BA_SPMV_SMEM")) g_ba_spmv_smem = atoi(e) != 0;
   double last_gmax = 0.0;
   int discarded_pcg = 0;

@@ -2,11 +2,13 @@
 //
 // Reference behaviour: src/colmap/mvs/patch_match_cuda.cu (PatchMatchCuda).  Design (DESIGN.md §2):
 //   * no physical Rotate() between sweeps (patch_match_cuda.cu:1859-1939): the four sweep
-//     directions are index maps over buffers that stay in the original orientation;
-//   * one CTA per image column (in the sweep's frame), WPC warps per CTA: warp 0 carries the
-//     sequential state of the column (PRNG, propagated plane, HMM forward messages), all warps share
-//     the photo-consistency work; each NCC is evaluated by an 8-lane group, the four groups of a warp
-//     being the four alternative plane hypotheses of SweepFromTopToBottom (:1117-1126);
+//     directions are index maps (frames) over buffers that stay in the original orientation;
+//   * each sweep runs as four passes: R draws every row's random hypothesis and Monte-Carlo uniforms
+//     from the column's PRNG stream, M (beside R) computes the column's HMM messages over the
+//     sweep-start costs, P evaluates pixel-parallel everything that does not depend on the row above,
+//     and S, one CTA of WPC warps per column, carries the column's sequential state (propagated plane,
+//     forward messages, sampling, argmin, filter);
+//   * each NCC is evaluated by an 8-lane group, so a warp runs four (hypothesis, image) pairs at once;
 //   * bilateral weights are computed once per pixel (they only depend on the reference patch) instead
 //     of once per NCC evaluation, and each (hypothesis, source image) pair is evaluated once per pixel
 //     instead of once per Monte-Carlo sample (NCC is a pure function of the pair);
@@ -79,7 +81,9 @@ struct PmSweepArgs {
                            // predicts which images the serial pass will sample from them
   int prune;               // 0: the pixel pass evaluates every (hypothesis, image) pair; 1: prediction + exact early-out;
                            // 2: (tests) the pixel pass evaluates nothing, the serial pass fills every entry itself
-  int col0, col1;          // column range [col0, col1) of the sweep frame handled by this launch (pixel / serial pass)
+  int col0;                // always 0; pm_serial_kernel reads its column as col0 + blockIdx.x because with blockIdx.x
+                           // alone the compiler schedules the row loop differently and the serial pass measured ~0.7 ms
+                           // per C2 sweep slower (H100 80GB HBM3 SXM, 400 W power limit)
 };
 #define PM_NOT_EVALUATED (-1.0f)   // tab3 sentinel (an NCC cost is always in [0, 2])
 
@@ -366,269 +370,13 @@ __global__ void __launch_bounds__(128) pm_initial_cost_kernel(const PmParams P) 
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// SweepFromTopToBottom (patch_match_cuda.cu:933-1288): one CTA per column of the sweep frame.
-// ------------------------------------------------------------------------------------------------
-template <int WPC, bool GEOM>
-__global__ void __launch_bounds__(32 * WPC) pm_sweep_kernel(const PmParams P, const PmSweepArgs A) {
-  extern __shared__ float4 smem4[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int col = blockIdx.x;
-  const int rot = A.rot, N = P.N;
-  const int fw = (rot & 1) ? P.H0 : P.W0, fh = (rot & 1) ? P.W0 : P.H0;
-
-  float4* patch = smem4;
-  float* poses = reinterpret_cast<float*>(patch + P.ntaps_pad);
-  float* tab = poses + N * PM_POSE_STRIDE;  // [5][32] cost of hypothesis k for image i (k = 0: cached cost)
-  float* gtab = tab + 160;                  // [3][32] geometric cost at cur / prev / rand depth
-  float* hyp = gtab + 96;                   // [5][4]  depth, normal of the five hypotheses (:1117-1126)
-  float* fctl = hyp + 20;                   // inv_wsum, ref_sum, ref_sqsum
-  int* ctrl = reinterpret_cast<int*>(fctl + 4);  // needed, remaining, best
-  int* samples = ctrl + 4;                  // [num_samples]
-
-  for (int i = threadIdx.x; i < N * PM_POSE_STRIDE; i += blockDim.x) poses[i] = P.poses[(size_t)rot * N * PM_POSE_STRIDE + i];
-  pm_fill_tap_offsets(P, patch, threadIdx.x, blockDim.x);
-  const float iK[4] = {P.invK[rot][0], P.invK[rot][1], P.invK[rot][2], P.invK[rot][3]};
-  const float Kr[4] = {P.K[rot][0], P.K[rot][1], P.K[rot][2], P.K[rot][3]};
-  const float colf = (float)col;
-  const int g = lane >> 3, sub = lane & 7;
-  const unsigned gmask = 0xffu << (8 * g);
-  const bool img_lane = lane < N;
-  const unsigned nmask = (N >= 32) ? 0xffffffffu : ((1u << N) - 1u);
-  __syncthreads();
-
-  // ---- backward messages for the whole column (:976-989); lane = image
-  float fwd = 0.5f;
-  PmRng rs;
-  float prev_d = 0.0f, prev_n0 = 0.0f, prev_n1 = 0.0f, prev_n2 = 0.0f;
-  uint32_t* rng_slot = nullptr;
-  if (warp == 0) {
-    if (img_lane) {
-      float beta = 0.5f;
-      for (int row = fh - 1; row >= 0; --row) {
-        const size_t p = pm_pix0(P.W0, P.H0, rot, row, col);
-        beta = pm_backward_message(P.L, P.cost[p * N + lane], beta);
-        A.sel_cur[p * N + lane] = beta;
-      }
-    }
-    int r0, c0;
-    pm_frame_to_orig(P.W0, P.H0, rot, 0, col, &r0, &c0);
-    rng_slot = P.rng + 6 * (size_t)pm_border_index(P.W0, P.H0, r0, c0);
-    rs.v0 = rng_slot[0]; rs.v1 = rng_slot[1]; rs.v2 = rng_slot[2]; rs.v3 = rng_slot[3]; rs.v4 = rng_slot[4]; rs.d = rng_slot[5];
-    const float4 h0 = P.hyp[(size_t)r0 * P.W0 + c0];
-    prev_d = h0.x; prev_n0 = h0.y; prev_n1 = h0.z; prev_n2 = h0.w;
-    pm_normal_to_frame(rot, prev_n0, prev_n1);
-  }
-
-  for (int row = 0; row < fh; ++row) {
-    const size_t p = pm_pix0(P.W0, P.H0, rot, row, col);
-    const float rowf = (float)row;
-
-    // ---- reference patch (one warp), overlapped with phase A on warp 0 when WPC > 1
-    if (warp == WPC - 1) {
-      float inv_wsum;
-      pm_build_patch(P, rot, fw, fh, row, col, patch, lane, &inv_wsum);
-      if (lane == 0) { fctl[0] = inv_wsum; fctl[1] = P.ref_sum[p]; fctl[2] = P.ref_sqsum[p]; }
-    }
-
-    // ---- phase A (warp 0): hypotheses, sampling distribution, Monte-Carlo samples
-    float cost_i = 0.0f, beta_i = 0.0f, prevp_i = 0.0f, rx = 0.0f, ry = 0.0f;
-    if (warp == 0) {
-      prev_d = pm_propagate_depth(iK, prev_d, prev_n1, prev_n2, (float)(row - 1), rowf);
-      const float4 cur4 = P.hyp[p];
-      const float cur_d = cur4.x;
-      float cur_n0 = cur4.y, cur_n1 = cur4.z;
-      const float cur_n2 = cur4.w;
-      pm_normal_to_frame(rot, cur_n0, cur_n1);
-      float rand_d, rand_n[3];
-      {
-        const float dmin = (1.0f - A.perturbation) * cur_d;
-        const float dmax = (1.0f + A.perturbation) * cur_d;
-        rand_d = fmaf(pm_rng_uniform(rs), dmax - dmin, dmin);
-      }
-      pm_perturb_normal(iK, rowf, colf, A.perturbation_pi, cur_n0, cur_n1, cur_n2, rs, rand_n);
-      rx = fmaf(iK[0], colf, iK[1]);
-      ry = fmaf(iK[2], rowf, iK[3]);
-      float prob = 0.0f;
-      if (img_lane) {
-        const float* pose = poses + lane * PM_POSE_STRIDE;
-        cost_i = P.cost[p * N + lane];
-        beta_i = A.sel_cur[p * N + lane];
-        prevp_i = A.sel_prev[p * N + lane];
-        const float alpha = pm_forward_message(P.L, cost_i, fwd);
-        const float sp = pm_sel_prob(alpha, beta_i, prevp_i, A.prev_w);
-        float ct, ci;
-        pm_viewing_angles(pose, cur_d * rx, cur_d * ry, cur_d, cur_n0, cur_n1, cur_n2, &ct, &ci);
-        float Hm[9];
-        pm_compose_homography(pose, iK, rowf, colf, cur_d, cur_n0, cur_n1, cur_n2, Hm);
-        prob = sp * pm_tri_prob(P.L, ct) * pm_inc_prob(P.L, ci) * pm_res_prob(Hm, rowf, colf, P.radius);
-        tab[lane] = cost_i;
-      }
-      // TransformPDFToCDF (:683-696)
-      float sum = 0.0f;
-      for (int i = 0; i < N; ++i) sum += __shfl_sync(0xffffffffu, prob, i);
-      const float inv = 1.0f / sum;
-      float cum = 0.0f, cdf = 0.0f;
-      for (int i = 0; i < N; ++i) {
-        cum += __shfl_sync(0xffffffffu, prob, i) * inv;
-        if (lane == i) cdf = cum;
-      }
-      unsigned needed = 0u;
-      for (int s = 0; s < P.num_samples; ++s) {
-        const float u = pm_rng_uniform(rs) - FLT_EPSILON;
-        const unsigned m = __ballot_sync(0xffffffffu, img_lane && (cdf > u));
-        const int img = m ? (__ffs(m) - 1) : -1;
-        if (lane == 0) samples[s] = img;
-        if (img >= 0) needed |= 1u << img;
-      }
-      if (lane == 0) {
-        ctrl[0] = (int)needed;
-        hyp[0] = cur_d;  hyp[1] = cur_n0;  hyp[2] = cur_n1;  hyp[3] = cur_n2;
-        hyp[4] = prev_d; hyp[5] = prev_n0; hyp[6] = prev_n1; hyp[7] = prev_n2;
-        hyp[8] = rand_d; hyp[9] = rand_n[0]; hyp[10] = rand_n[1]; hyp[11] = rand_n[2];
-        hyp[12] = cur_d; hyp[13] = rand_n[0]; hyp[14] = rand_n[1]; hyp[15] = rand_n[2];
-        hyp[16] = rand_d; hyp[17] = cur_n0; hyp[18] = cur_n1; hyp[19] = cur_n2;
-      }
-      if (GEOM) {
-        if (img_lane && ((needed >> lane) & 1u)) {
-          const PmSrcDesc sd = P.src[lane];
-          const float* pose = poses + lane * PM_POSE_STRIDE;
-          const float* dm = P.src_depth + sd.depth_off;
-          gtab[lane] = pm_geom_cost(pose, Kr, iK, dm, sd.w, sd.h, rowf, colf, cur_d, P.geom_max_cost);
-          gtab[32 + lane] = pm_geom_cost(pose, Kr, iK, dm, sd.w, sd.h, rowf, colf, prev_d, P.geom_max_cost);
-          gtab[64 + lane] = pm_geom_cost(pose, Kr, iK, dm, sd.w, sd.h, rowf, colf, rand_d, P.geom_max_cost);
-        }
-      }
-    }
-    __syncthreads();  // #1: patch, hypotheses, samples visible
-
-    // ---- phase B (all warps): NCC of the four alternative hypotheses for every sampled image
-    const float inv_wsum = fctl[0], rsum = fctl[1], rsq = fctl[2];
-    {
-      const unsigned needed = (unsigned)ctrl[0];
-      const int h = g + 1;
-      const float hd = hyp[4 * h], hn0 = hyp[4 * h + 1], hn1 = hyp[4 * h + 2], hn2 = hyp[4 * h + 3];
-      int k = 0;
-      for (unsigned m = needed; m; m &= m - 1, ++k) {
-        if ((k % WPC) != warp) continue;
-        const int img = __ffs(m) - 1;
-        const PmSrcDesc sd = P.src[img];
-        const float c = pm_ncc_group(patch, P.ntaps, poses + img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch,
-                                     sd.w, sd.h, rowf, colf, hd, hn0, hn1, hn2, inv_wsum, rsum, rsq, sub, gmask);
-        if (sub == 0) tab[h * 32 + img] = c;
-      }
-    }
-    __syncthreads();  // #2: cost table complete
-
-    // ---- phase C (warp 0): accumulate sampled costs, pick the best hypothesis (:1128-1182)
-    int best = 0;
-    if (warp == 0) {
-      float c = 0.0f;
-      if (lane < 5) {
-        const int gi = (lane == 1) ? 1 : ((lane == 2 || lane == 4) ? 2 : 0);
-        for (int s = 0; s < P.num_samples; ++s) {
-          const int img = samples[s];
-          if (img < 0) continue;
-          c += tab[lane * 32 + img];
-          if (GEOM) c = fmaf(P.geom_reg, gtab[gi * 32 + img], c);
-        }
-      }
-      float mn = __shfl_sync(0xffffffffu, c, 0);
-      for (int k = 1; k < 5; ++k) {
-        const float ck = __shfl_sync(0xffffffffu, c, k);
-        if (ck <= mn) { mn = ck; best = k; }
-      }
-      if (lane == 0) {
-        const unsigned needed = (unsigned)ctrl[0];
-        ctrl[1] = (best == 0) ? 0 : (int)(~needed & nmask);
-        ctrl[2] = best;
-      }
-    }
-    __syncthreads();  // #3: best / remaining visible
-
-    // ---- phase D (all warps): cost of the winning hypothesis for the images that were not sampled
-    {
-      const unsigned remaining = (unsigned)ctrl[1];
-      if (remaining) {
-        const int b = ctrl[2];
-        const float hd = hyp[4 * b], hn0 = hyp[4 * b + 1], hn1 = hyp[4 * b + 2], hn2 = hyp[4 * b + 3];
-        const int item = warp * 4 + g;
-        int k = 0;
-        for (unsigned m = remaining; m; m &= m - 1, ++k) {
-          if ((k % (4 * WPC)) != item) continue;
-          const int img = __ffs(m) - 1;
-          const PmSrcDesc sd = P.src[img];
-          const float c = pm_ncc_group(patch, P.ntaps, poses + img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off,
-                                       sd.pitch, sd.w, sd.h, rowf, colf, hd, hn0, hn1, hn2, inv_wsum, rsum, rsq, sub,
-                                       gmask);
-          if (sub == 0) tab[b * 32 + img] = c;
-        }
-      }
-    }
-    __syncthreads();  // #4
-
-    // ---- phase E (warp 0): new messages / selection probabilities, filter, carry state (:1184-1283)
-    if (warp == 0) {
-      const float best_d = hyp[4 * best];
-      const float bn0 = hyp[4 * best + 1], bn1 = hyp[4 * best + 2], bn2 = hyp[4 * best + 3];
-      float sp = 0.0f;
-      if (img_lane) {
-        float c = cost_i;
-        if (best != 0) {
-          c = tab[best * 32 + lane];
-          P.cost[p * N + lane] = c;
-        }
-        const float alpha = pm_forward_message(P.L, c, fwd);
-        sp = pm_sel_prob(alpha, beta_i, prevp_i, A.prev_w);
-        A.sel_cur[p * N + lane] = sp;
-        fwd = alpha;
-      }
-      bool zero = false;
-      if (A.last_filter) {
-        bool ok = false;
-        if (img_lane) {
-          const float* pose = poses + lane * PM_POSE_STRIDE;
-          float ct, ci;
-          pm_viewing_angles(pose, best_d * rx, best_d * ry, best_d, bn0, bn1, bn2, &ct, &ci);
-          if (!(ct > P.cos_filter_tri || ci <= 0.0f)) {
-            ok = sp >= P.min_ncc_prob;
-            if (GEOM && ok) {
-              const PmSrcDesc sd = P.src[lane];
-              ok = pm_geom_cost(pose, Kr, iK, P.src_depth + sd.depth_off, sd.w, sd.h, rowf, colf, best_d,
-                                P.geom_max_cost) <= P.filter_geom_max_cost;
-            }
-          }
-        }
-        const int cnt = __popc(__ballot_sync(0xffffffffu, ok));
-        zero = cnt < P.filter_min_num_consistent;
-        if (img_lane) P.mask[p * N + lane] = (ok && !zero) ? 1 : 0;
-      }
-      if (lane == 0) {
-        float o0 = bn0, o1 = bn1;
-        pm_normal_to_orig(rot, o0, o1);
-        if (zero) {
-          // the reference stores +0 in the sweep frame and then rotates (:1268-1271)
-          float z0 = 0.0f, z1 = 0.0f;
-          pm_normal_to_orig(rot, z0, z1);
-          P.hyp[p] = make_float4(0.0f, z0, z1, 0.0f);
-        } else {
-          P.hyp[p] = make_float4(best_d, o0, o1, bn2);
-        }
-      }
-      prev_d = best_d; prev_n0 = bn0; prev_n1 = bn1; prev_n2 = bn2;
-    }
-  }
-  if (warp == 0 && lane == 0) {
-    rng_slot[0] = rs.v0; rng_slot[1] = rs.v1; rng_slot[2] = rs.v2; rng_slot[3] = rs.v3; rng_slot[4] = rs.v4; rng_slot[5] = rs.d;
-  }
-}
-
-
 // ================================================================================================
-// Split sweep (default): the same SweepFromTopToBottom semantics in three passes.
+// Sweep: SweepFromTopToBottom (patch_match_cuda.cu:933-1288) in four passes.
 //   R  pm_rand_kernel    column-serial, one thread per column: consumes the column's XORWOW stream to
 //                        produce every row's random hypothesis (the stream position of a row does not
 //                        depend on the sweep's results, only on the hypotheses of the previous sweep);
+//   M  pm_msg_kernel     one thread per (column, image), beside R: the column's HMM messages over the
+//                        costs the sweep starts with;
 //   P  pm_pixel_kernel   pixel-parallel, one warp per pixel: everything that does not depend on the row
 //                        above — the NCC of hypotheses 2..4 (rand/rand, cur/rand-normal, rand-depth/cur)
 //                        against every source image, the per-image priors, geometric costs;
@@ -711,8 +459,8 @@ __global__ void pm_msg_kernel(const PmParams P, const PmSweepArgs A) {
 //   * entries it did not evaluate stay PM_NOT_EVALUATED.
 // Exactness does not depend on the prediction: pm_serial_kernel re-checks "partial sum > cost sum of hypothesis 0"
 // with the true samples in the true summation order and evaluates any entry it really needs itself.
-template <bool GEOM, bool PRUNE, int MINB>
-__global__ void __launch_bounds__(128, MINB) pm_pixel_kernel(const PmParams P, const PmSweepArgs A) {
+template <bool GEOM, bool PRUNE>
+__global__ void __launch_bounds__(128, 8) pm_pixel_kernel(const PmParams P, const PmSweepArgs A) {
   extern __shared__ float4 smem4[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rot = A.rot, N = P.N;
@@ -724,8 +472,7 @@ __global__ void __launch_bounds__(128, MINB) pm_pixel_kernel(const PmParams P, c
   const float iK[4] = {P.invK[rot][0], P.invK[rot][1], P.invK[rot][2], P.invK[rot][3]};
   const float Kr[4] = {P.K[rot][0], P.K[rot][1], P.K[rot][2], P.K[rot][3]};
   __syncthreads();
-  const int cw = A.col1 - A.col0;
-  const size_t npix = (size_t)cw * fh;
+  const size_t npix = (size_t)fw * fh;
   const int g = lane >> 3, sub = lane & 7;
   const unsigned gmask = 0xffu << (8 * g);
   const unsigned full = 0xffffffffu;
@@ -735,7 +482,7 @@ __global__ void __launch_bounds__(128, MINB) pm_pixel_kernel(const PmParams P, c
   (void)fw; (void)nsl; (void)full; (void)nmask;
   // (an SM-local tiling of the pixel order was measured: L1 hit rate 67% -> 55%, slower; plain grid stride kept)
   for (size_t q = (size_t)blockIdx.x * 4 + warp; q < npix; q += (size_t)gridDim.x * 4) {
-    const int row = (int)(q / cw), col = A.col0 + (int)(q - (size_t)row * cw);  // sweep-frame pixel
+    const int row = (int)(q / fw), col = (int)(q - (size_t)row * fw);  // sweep-frame pixel
     const size_t p = pm_pix0(P.W0, P.H0, rot, row, col);
     const float rowf = (float)row, colf = (float)col;
     float inv_wsum;
@@ -869,8 +616,8 @@ __global__ void __launch_bounds__(128, MINB) pm_pixel_kernel(const PmParams P, c
   }
 }
 
-template <int WPC, bool GEOM, int MINB>
-__global__ void __launch_bounds__(32 * WPC, MINB) pm_serial_kernel(const PmParams P, const PmSweepArgs A) {
+template <int WPC, bool GEOM>
+__global__ void __launch_bounds__(32 * WPC, 16 / WPC) pm_serial_kernel(const PmParams P, const PmSweepArgs A) {
   extern __shared__ float4 smem4[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int col = A.col0 + blockIdx.x;
@@ -1182,16 +929,10 @@ struct b200pm_context {
   int device = 0;
   int wpc = 2;
   bool wpc_auto = true;   // B200PM_WPC unset: the serial pass picks its schedule per sweep (one wave of columns)
-  bool serial_cap = false; // B200PM_SERIAL_CAP=1: allow the register-capped (72 regs, 13 CTAs/SM, small spills) WPC = 2 variant
   int num_sms = 132;
   cudaStream_t stream = nullptr;
   cudaStream_t stream2 = nullptr;     // pass M runs here, next to pass R on the main stream
-  std::vector<cudaStream_t> chunk_stream;   // one high-priority stream per column chunk for the serial pass
-  int pix_minb = 8;                   // resident pixel-pass CTAs per SM the kernel is compiled for (B200PM_PIX_MINB = 6 | 7 | 8)
-  int pix_per_warp = 4;               // pixels a pixel-pass warp handles before its CTA retires (B200PM_PPW; 4 is the fastest on H100)
-  std::vector<cudaEvent_t> chunk_ev;  // pixel chunk i done (main stream) ; [kMaxChunks] = serial pass of the sweep done
-  int chunks = 1;                     // column chunks per sweep (B200PM_CHUNKS); more than one chunk was slower at C2
-                                      // (the 128-register serial CTAs starve the pixel pass of registers)
+  cudaEvent_t fork_ev = nullptr, join_ev = nullptr;   // main stream -> pass M on stream2 -> main stream
   int prune = 1, prune_from = 1;      // exact early-out in the pixel pass (B200PM_PRUNE), from this sweep on (B200PM_PRUNE_FROM)
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
   std::vector<std::pair<void*, size_t>> allocs;
@@ -1199,16 +940,16 @@ struct b200pm_context {
   int final_sel = 0;
   bool dirty = false, ran = false;
   float last_ms = 0.0f, last_sweep_ms = 0.0f;
-  float last_kernel_ms[3] = {0.0f, 0.0f, 0.0f};  // rand / pixel / serial(or fused) passes of the last run
+  float last_kernel_ms[3] = {0.0f, 0.0f, 0.0f};  // rand(+msg) / pixel / serial passes of the last run
   std::vector<cudaEvent_t> sweep_ev;
   int last_launches = 0;
   std::vector<int> src_image_idxs;
-  size_t smem_sweep = 0, smem_init = 0, smem_serial = 0;
-  bool fused = false;
+  size_t smem_init = 0, smem_serial = 0;
   float4* rand_hyp = nullptr; unsigned char* ntrials = nullptr; float* usamp = nullptr; float* prior3 = nullptr; float* tab3 = nullptr; float* gtab2 = nullptr;
   float* fwd_pred = nullptr;
 };
-#define PM_MAX_CHUNKS 16
+// pixels a pixel-pass warp handles before its CTA retires (4 measured fastest on the H100; 8 was ~7 ms per C2 run slower)
+#define PM_PIXELS_PER_WARP 4
 
 template <typename T>
 static cudaError_t pm_alloc(b200pm_context* c, T** p, size_t count) {
@@ -1354,22 +1095,17 @@ int b200pm_create(const b200pm_options* o, const b200pm_problem* p, b200pm_handl
   PM_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
   for (int i = 0; i < 4; ++i) PM_CUDA(cudaEventCreate(&c->ev[i]));
   PM_CUDA(cudaStreamCreateWithFlags(&c->stream2, cudaStreamNonBlocking));
-  {
-    int lo = 0, hi = 0;
-    cudaDeviceGetStreamPriorityRange(&lo, &hi);   // hi = numerically lowest = highest priority
-    c->chunk_stream.resize(PM_MAX_CHUNKS);
-    for (auto& st : c->chunk_stream) PM_CUDA(cudaStreamCreateWithPriority(&st, cudaStreamNonBlocking, hi));
-  }
-  if (const char* e = getenv("B200PM_PIX_MINB")) { const int v = atoi(e); if (v >= 6 && v <= 8) c->pix_minb = v; }
-  if (const char* e = getenv("B200PM_PPW")) c->pix_per_warp = std::max(1, atoi(e));
-  c->chunk_ev.resize(2 * PM_MAX_CHUNKS + 2);
-  for (auto& e : c->chunk_ev) PM_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  if (const char* e = getenv("B200PM_CHUNKS")) c->chunks = std::max(1, std::min(PM_MAX_CHUNKS, atoi(e)));
+  PM_CUDA(cudaEventCreateWithFlags(&c->fork_ev, cudaEventDisableTiming));
+  PM_CUDA(cudaEventCreateWithFlags(&c->join_ev, cudaEventDisableTiming));
+  // Test and diagnostic seams; none changes the result.  B200PM_WPC forces the serial pass's warps per column (the
+  // automatic choice depends on the column count against the SM count, so small problems never reach WPC = 1 without
+  // it); B200PM_PRUNE / B200PM_PRUNE_FROM select the pixel pass's early-out schedule (PRUNE=2 evaluates nothing there,
+  // which shows the serial pass does not depend on the prediction); B200PM_MAX_SWEEPS (read per run by b200pm_run)
+  // stops a run after that many sweeps, for sweep-by-sweep comparison with the oracle.
   if (const char* e = getenv("B200PM_PRUNE")) c->prune = atoi(e);
   if (const char* e = getenv("B200PM_PRUNE_FROM")) c->prune_from = atoi(e);
   if (const char* e = getenv("B200PM_WPC")) { c->wpc = atoi(e); c->wpc_auto = false; }
   if (c->wpc != 1 && c->wpc != 2 && c->wpc != 4) c->wpc = 2;
-  if (const char* e = getenv("B200PM_SERIAL_CAP")) c->serial_cap = atoi(e) != 0;
   cudaDeviceGetAttribute(&c->num_sms, cudaDevAttrMultiProcessorCount, c->device);
 
   PmParams& P = c->P;
@@ -1465,20 +1201,15 @@ int b200pm_create(const b200pm_options* o, const b200pm_problem* p, b200pm_handl
     pm_prefilter_kernel<<<grd, blk, 0, s>>>(P);
     pm_init_kernel<<<grd, blk, 0, s>>>(P, c->sel[1]);
   }
-  c->smem_sweep = sizeof(float4) * P.ntaps_pad + sizeof(float) * ((size_t)N * PM_POSE_STRIDE + 160 + 96 + 20 + 4) +
-                  sizeof(int) * (4 + (size_t)P.num_samples);
   c->smem_init = sizeof(float4) * 4 * P.ntaps_pad + sizeof(float) * (size_t)N * PM_POSE_STRIDE;
   c->smem_serial = sizeof(float4) * 2 * P.ntaps_pad + sizeof(float) * ((size_t)N * PM_POSE_STRIDE + 32 + 4 + 8 + 272);
-  c->fused = getenv("B200PM_FUSED") != nullptr && atoi(getenv("B200PM_FUSED")) != 0;
-  if (!c->fused) {
-    PM_CUDA(pm_alloc(c, &c->rand_hyp, n));
-    PM_CUDA(pm_alloc(c, &c->ntrials, n));
-    PM_CUDA(pm_alloc(c, &c->usamp, n * (size_t)o->num_samples));
-    PM_CUDA(pm_alloc(c, &c->prior3, 3 * n * N));
-    PM_CUDA(pm_alloc(c, &c->tab3, 3 * n * N));
-    if (P.geom) PM_CUDA(pm_alloc(c, &c->gtab2, 2 * n * N));
-    PM_CUDA(pm_alloc(c, &c->fwd_pred, n * N));
-  }
+  PM_CUDA(pm_alloc(c, &c->rand_hyp, n));
+  PM_CUDA(pm_alloc(c, &c->ntrials, n));
+  PM_CUDA(pm_alloc(c, &c->usamp, n * (size_t)o->num_samples));
+  PM_CUDA(pm_alloc(c, &c->prior3, 3 * n * N));
+  PM_CUDA(pm_alloc(c, &c->tab3, 3 * n * N));
+  if (P.geom) PM_CUDA(pm_alloc(c, &c->gtab2, 2 * n * N));
+  PM_CUDA(pm_alloc(c, &c->fwd_pred, n * N));
   PM_CUDA(cudaStreamSynchronize(s));
   PM_CUDA(cudaGetLastError());
   *out = c;
@@ -1488,23 +1219,15 @@ int b200pm_create(const b200pm_options* o, const b200pm_problem* p, b200pm_handl
 }  // extern "C"
 
 template <int WPC>
-static void pm_launch_sweep(b200pm_context* c, const PmSweepArgs& A, int fw) {
-  if (c->P.geom)
-    pm_sweep_kernel<WPC, true><<<fw, 32 * WPC, c->smem_sweep, c->stream>>>(c->P, A);
-  else
-    pm_sweep_kernel<WPC, false><<<fw, 32 * WPC, c->smem_sweep, c->stream>>>(c->P, A);
-}
-template <int WPC, int MINB>
-static void pm_launch_serial(b200pm_context* c, const PmSweepArgs& A, cudaStream_t st) {
-  const int cw = A.col1 - A.col0;
+static void pm_launch_serial(b200pm_context* c, const PmSweepArgs& A, int fw) {
   if (c->smem_serial > 48 * 1024) {
-    cudaFuncSetAttribute(pm_serial_kernel<WPC, true, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_serial);
-    cudaFuncSetAttribute(pm_serial_kernel<WPC, false, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_serial);
+    cudaFuncSetAttribute(pm_serial_kernel<WPC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_serial);
+    cudaFuncSetAttribute(pm_serial_kernel<WPC, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_serial);
   }
   if (c->P.geom)
-    pm_serial_kernel<WPC, true, MINB><<<cw, 32 * WPC, c->smem_serial, st>>>(c->P, A);
+    pm_serial_kernel<WPC, true><<<fw, 32 * WPC, c->smem_serial, c->stream>>>(c->P, A);
   else
-    pm_serial_kernel<WPC, false, MINB><<<cw, 32 * WPC, c->smem_serial, st>>>(c->P, A);
+    pm_serial_kernel<WPC, false><<<fw, 32 * WPC, c->smem_serial, c->stream>>>(c->P, A);
 }
 
 extern "C" {
@@ -1515,20 +1238,12 @@ int b200pm_run(b200pm_handle c) {
   PM_CUDA(cudaSetDevice(c->device));
   const PmParams& P = c->P;
   cudaStream_t s = c->stream;
-  if (c->smem_sweep > 48 * 1024) {
-    PM_CUDA(cudaFuncSetAttribute(pm_sweep_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_sweep));
-    PM_CUDA(cudaFuncSetAttribute(pm_sweep_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_sweep));
-    PM_CUDA(cudaFuncSetAttribute(pm_sweep_kernel<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_sweep));
-    PM_CUDA(cudaFuncSetAttribute(pm_sweep_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_sweep));
-    PM_CUDA(cudaFuncSetAttribute(pm_sweep_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_sweep));
-    PM_CUDA(cudaFuncSetAttribute(pm_sweep_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_sweep));
-  }
   if (c->smem_init > 48 * 1024) {
     PM_CUDA(cudaFuncSetAttribute(pm_initial_cost_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_init));
-#define PM_ATTR(G, PR, MB) PM_CUDA(cudaFuncSetAttribute(pm_pixel_kernel<G, PR, MB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_init))
-    PM_ATTR(false, false, 8); PM_ATTR(true, false, 8); PM_ATTR(false, true, 8); PM_ATTR(true, true, 8);
-    PM_ATTR(false, true, 7); PM_ATTR(true, true, 7); PM_ATTR(false, true, 6); PM_ATTR(true, true, 6);
-#undef PM_ATTR
+    PM_CUDA(cudaFuncSetAttribute(pm_pixel_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_init));
+    PM_CUDA(cudaFuncSetAttribute(pm_pixel_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_init));
+    PM_CUDA(cudaFuncSetAttribute(pm_pixel_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_init));
+    PM_CUDA(cudaFuncSetAttribute(pm_pixel_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_init));
   }
   int launches = 0;
   PM_CUDA(cudaEventRecord(c->ev[0], s));
@@ -1568,71 +1283,38 @@ int b200pm_run(b200pm_handle c) {
         cudaEventRecord(c->sweep_ev[id], s);
       };
       mark(0);
-      if (c->fused) {
-        if (c->wpc == 1) pm_launch_sweep<1>(c, A, fw);
-        else if (c->wpc == 2) pm_launch_sweep<2>(c, A, fw);
-        else pm_launch_sweep<4>(c, A, fw);
-        ++launches;
-        mark(1); mark(2); mark(3);
+      A.rand_hyp = c->rand_hyp; A.ntrials = c->ntrials; A.usamp = c->usamp; A.prior3 = c->prior3; A.tab3 = c->tab3; A.gtab2 = c->gtab2;
+      A.fwd_pred = c->fwd_pred;
+      A.prune = (c->prune == 1) ? ((t >= c->prune_from) ? 1 : 0) : c->prune;
+      // pass M (messages) runs beside pass R (random hypotheses): both only read the state the last sweep left
+      cudaEventRecord(c->fork_ev, s);
+      cudaStreamWaitEvent(c->stream2, c->fork_ev, 0);
+      pm_msg_kernel<<<(fw * P.N + 127) / 128, 128, 0, c->stream2>>>(P, A);
+      cudaEventRecord(c->join_ev, c->stream2);
+      pm_rand_kernel<<<(fw + 63) / 64, 64, 0, s>>>(P, A);
+      cudaStreamWaitEvent(s, c->join_ev, 0);
+      mark(1);
+      const size_t npx = (size_t)fw * ((sweep & 1) ? P.W0 : P.H0);
+      const int pgrid = (int)((npx + 4 * PM_PIXELS_PER_WARP - 1) / (4 * PM_PIXELS_PER_WARP));
+      if (P.geom) {
+        if (A.prune) pm_pixel_kernel<true, true><<<pgrid, 128, c->smem_init, s>>>(P, A);
+        else pm_pixel_kernel<true, false><<<pgrid, 128, c->smem_init, s>>>(P, A);
       } else {
-        A.rand_hyp = c->rand_hyp; A.ntrials = c->ntrials; A.usamp = c->usamp; A.prior3 = c->prior3; A.tab3 = c->tab3; A.gtab2 = c->gtab2;
-        A.fwd_pred = c->fwd_pred;
-        A.prune = (c->prune == 1) ? ((t >= c->prune_from) ? 1 : 0) : c->prune;
-        A.col0 = 0; A.col1 = fw;
-        // pass M (messages) runs beside pass R (random hypotheses): both only read the state the last sweep left
-        cudaEventRecord(c->chunk_ev[2 * PM_MAX_CHUNKS], s);
-        cudaStreamWaitEvent(c->stream2, c->chunk_ev[2 * PM_MAX_CHUNKS], 0);
-        pm_msg_kernel<<<(fw * P.N + 127) / 128, 128, 0, c->stream2>>>(P, A);
-        cudaEventRecord(c->chunk_ev[2 * PM_MAX_CHUNKS + 1], c->stream2);
-        pm_rand_kernel<<<(fw + 63) / 64, 64, 0, s>>>(P, A);
-        cudaStreamWaitEvent(s, c->chunk_ev[2 * PM_MAX_CHUNKS + 1], 0);
-        mark(1);
-        // The serial pass is one CTA per column marching down all rows: a second wave of CTAs lengthens its critical
-        // path.  Pick the widest schedule whose resident capacity covers all fw columns in ONE wave (register-file
-        // bound: 128 registers x 32*WPC threads per CTA).  On the H100 (132 SMs) every C2 sweep, 1920 or 1080 columns,
-        // runs WPC = 1 (a fixed WPC = 2 is ~18 ms per run slower).
-        int wpc = c->wpc, capped = 0;
-        if (c->wpc_auto) {
-          const int sms = c->num_sms;
-          if (fw <= sms * 4) wpc = 4;
-          else if (fw <= sms * 8) wpc = 2;
-          else if (fw <= sms * 13 && c->serial_cap) { wpc = 2; capped = 1; }
-          else wpc = 1;
-        }
-        // Columns are independent inside a sweep: the pixel pass runs in column chunks on the main stream (short-lived
-        // CTAs) and the serial pass of a chunk starts on its own high-priority stream as soon as its chunk is done, so
-        // the latency-bound serial pass overlaps the issue-bound pixel pass of the following chunks.
-        const int nchunks = std::max(1, std::min(c->chunks, fw / 32 > 0 ? fw / 32 : 1));
-        const int fh_ = (sweep & 1) ? P.W0 : P.H0;
-        for (int k = 0; k < nchunks; ++k) {
-          PmSweepArgs C = A;
-          C.col0 = (int)((long long)fw * k / nchunks); C.col1 = (int)((long long)fw * (k + 1) / nchunks);
-          const size_t npx = (size_t)(C.col1 - C.col0) * fh_;
-          const size_t per_cta = (size_t)4 * c->pix_per_warp;
-          const int pgrid = (int)((npx + per_cta - 1) / per_cta);
-          const bool pr = C.prune != 0;
-#define PM_LAUNCH_PIXEL(G, PR, MB) pm_pixel_kernel<G, PR, MB><<<pgrid, 128, c->smem_init, s>>>(P, C)
-          if (P.geom) { if (!pr) PM_LAUNCH_PIXEL(true, false, 8); else if (c->pix_minb == 8) PM_LAUNCH_PIXEL(true, true, 8); else if (c->pix_minb == 7) PM_LAUNCH_PIXEL(true, true, 7); else PM_LAUNCH_PIXEL(true, true, 6); }
-          else { if (!pr) PM_LAUNCH_PIXEL(false, false, 8); else if (c->pix_minb == 8) PM_LAUNCH_PIXEL(false, true, 8); else if (c->pix_minb == 7) PM_LAUNCH_PIXEL(false, true, 7); else PM_LAUNCH_PIXEL(false, true, 6); }
-#undef PM_LAUNCH_PIXEL
-          if (nchunks == 1) mark(2);   // pixel | serial boundary of the per-pass times (one chunk: both passes on the main stream)
-          cudaStream_t ss = nchunks > 1 ? c->chunk_stream[k] : s;
-          if (nchunks > 1) {
-            cudaEventRecord(c->chunk_ev[k], s);
-            cudaStreamWaitEvent(ss, c->chunk_ev[k], 0);
-          }
-          if (wpc == 1) pm_launch_serial<1, 16>(c, C, ss);
-          else if (wpc == 2 && capped) pm_launch_serial<2, 13>(c, C, ss);
-          else if (wpc == 2) pm_launch_serial<2, 8>(c, C, ss);
-          else pm_launch_serial<4, 4>(c, C, ss);
-          if (nchunks > 1) cudaEventRecord(c->chunk_ev[PM_MAX_CHUNKS + k], ss);
-          launches += 2;
-        }
-        if (nchunks > 1) mark(2);
-        if (nchunks > 1) for (int k = 0; k < nchunks; ++k) cudaStreamWaitEvent(s, c->chunk_ev[PM_MAX_CHUNKS + k], 0);
-        launches += 2;
-        mark(3);
+        if (A.prune) pm_pixel_kernel<false, true><<<pgrid, 128, c->smem_init, s>>>(P, A);
+        else pm_pixel_kernel<false, false><<<pgrid, 128, c->smem_init, s>>>(P, A);
       }
+      mark(2);
+      // The serial pass is one CTA per column marching down all rows: a second wave of CTAs lengthens its critical
+      // path.  Pick the widest schedule whose resident capacity covers all fw columns in ONE wave (register-file
+      // bound: 128 registers x 32*WPC threads per CTA).  On the H100 (132 SMs) every C2 sweep, 1920 or 1080 columns,
+      // runs WPC = 1 (a fixed WPC = 2 is ~18 ms per run slower).
+      int wpc = c->wpc;
+      if (c->wpc_auto) wpc = (fw <= c->num_sms * 4) ? 4 : ((fw <= c->num_sms * 8) ? 2 : 1);
+      if (wpc == 1) pm_launch_serial<1>(c, A, fw);
+      else if (wpc == 2) pm_launch_serial<2>(c, A, fw);
+      else pm_launch_serial<4>(c, A, fw);
+      launches += 4;
+      mark(3);
       c->final_sel = t & 1;
     }
   }
@@ -1737,8 +1419,8 @@ void b200pm_destroy(b200pm_handle c) {
   for (auto& a : c->allocs) B200DeviceCache::get().free(a.first, a.second);
   for (int i = 0; i < 4; ++i) if (c->ev[i]) cudaEventDestroy(c->ev[i]);
   for (cudaEvent_t e : c->sweep_ev) cudaEventDestroy(e);
-  for (cudaEvent_t e : c->chunk_ev) if (e) cudaEventDestroy(e);
-  for (cudaStream_t st : c->chunk_stream) if (st) { cudaStreamSynchronize(st); cudaStreamDestroy(st); }
+  if (c->fork_ev) cudaEventDestroy(c->fork_ev);
+  if (c->join_ev) cudaEventDestroy(c->join_ev);
   if (c->stream2) { cudaStreamSynchronize(c->stream2); cudaStreamDestroy(c->stream2); }
   if (c->stream) cudaStreamDestroy(c->stream);
   delete c;

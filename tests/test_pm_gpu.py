@@ -17,13 +17,12 @@ def _bits(a):
     return np.ascontiguousarray(a, np.float32).view(np.uint32)
 
 
-def _run_cuda(o, problem, wpc=None, fused=False, env=None):
+def _run_cuda(o, problem, wpc=None, env=None):
     for k, v in (env or {}).items():
         os.environ[k] = str(v)
     if wpc is not None:
         os.environ["B200PM_WPC"] = str(wpc)
     os.environ.pop("B200PM_MAX_SWEEPS", None)
-    os.environ["B200PM_FUSED"] = "1" if fused else "0"
     pm = PatchMatch(o, problem)
     pm.Run()
     out = dict(depth=pm.GetDepthMap(), normal=pm.GetNormalMap(), sel_prob=pm.GetSelProbMap())
@@ -32,7 +31,6 @@ def _run_cuda(o, problem, wpc=None, fused=False, env=None):
         out["list"] = pm.GetConsistentImageIdxs()
     pm.close()
     os.environ.pop("B200PM_WPC", None)
-    os.environ.pop("B200PM_FUSED", None)
     for k in (env or {}):
         os.environ.pop(k, None)
     return out
@@ -54,28 +52,27 @@ def test_fast_reciprocal_is_ieee_over_all_floats():
     assert lib.b200pm_test_rcp_exhaustive() == 0
 
 
-@pytest.mark.parametrize("wpc,fused", [(1, False), (2, False), (4, False), (1, True), (2, True), (4, True)])
-def test_photometric_bit_exact_vs_oracle(wpc, fused):
-    """Both schedules (split rand/pixel/serial passes = default, and the single fused sweep kernel) for every
-    warps-per-column setting must reproduce the oracle bit for bit."""
+@pytest.mark.parametrize("wpc", [1, 2, 4])
+def test_photometric_bit_exact_vs_oracle(wpc):
+    """Every warps-per-column schedule of the serial pass must reproduce the oracle bit for bit."""
     sc = make_patch_match_scene(96, 72, 4, seed=0)
     o = PatchMatchOptions(depth_min=sc["depth_min"], depth_max=sc["depth_max"], geom_consistency=False,
                           num_iterations=2)
-    got = _run_cuda(o, sc["problem"], wpc, fused)
+    got = _run_cuda(o, sc["problem"], wpc)
     ref = oracle_pm.run(o, sc["problem"])
     _assert_bit_exact(got, ref)
     assert np.array_equal(got["mask"], ref["mask"])
     assert np.array_equal(got["list"], consistency_list_from_mask(ref["mask"], sc["problem"].src_image_idxs))
 
 
-@pytest.mark.parametrize("prune,prune_from,chunks,geom", [
-    (0, 0, 1, False),     # the pixel pass evaluates every (hypothesis, image) pair, one chunk: the round-1 schedule
-    (1, 0, 3, False),     # prediction + exact early-out from the very first sweep (poor prediction: many late evaluations)
-    (1, 1, 4, False),     # the default schedule
-    (2, 0, 2, False),     # adversarial: the pixel pass evaluates NOTHING, the serial pass must fill every entry it needs
-    (1, 0, 2, True), (2, 0, 1, True),
+@pytest.mark.parametrize("prune,prune_from,geom", [
+    (0, 0, False),     # the pixel pass evaluates every (hypothesis, image) pair
+    (1, 0, False),     # prediction + exact early-out from the very first sweep (poor prediction: many late evaluations)
+    (1, 1, False),     # the default schedule
+    (2, 0, False),     # adversarial: the pixel pass evaluates NOTHING, the serial pass must fill every entry it needs
+    (1, 0, True), (2, 0, True),
 ])
-def test_early_out_schedules_are_exact(prune, prune_from, chunks, geom):
+def test_early_out_schedules_are_exact(prune, prune_from, geom):
     """The pixel pass may skip (hypothesis, image) pairs - predicted unsampled, or ruled out because the partial cost sum
     already exceeds the current hypothesis' - and the serial pass re-checks / fills in with the true samples.  Whatever the
     pixel pass chose to evaluate, the result must be the oracle's, bit for bit."""
@@ -89,7 +86,7 @@ def test_early_out_schedules_are_exact(prune, prune_from, chunks, geom):
                           num_samples=15 if not geom else 37)
     ref = oracle_pm.run(o, prob)
     for wpc in (1, 2):
-        got = _run_cuda(o, prob, wpc=wpc, env=dict(B200PM_PRUNE=prune, B200PM_PRUNE_FROM=prune_from, B200PM_CHUNKS=chunks))
+        got = _run_cuda(o, prob, wpc=wpc, env=dict(B200PM_PRUNE=prune, B200PM_PRUNE_FROM=prune_from))
         _assert_bit_exact(got, ref)
         assert np.array_equal(got["mask"], ref["mask"])
 
@@ -137,10 +134,9 @@ def test_geometric_consistency_bit_exact():
     o = PatchMatchOptions(depth_min=sc["depth_min"], depth_max=sc["depth_max"], geom_consistency=True,
                           num_iterations=1)
     ref = oracle_pm.run(o, prob)
-    for fused in (False, True):
-        got = _run_cuda(o, prob, fused=fused)
-        _assert_bit_exact(got, ref)
-        assert np.array_equal(got["mask"], ref["mask"])
+    got = _run_cuda(o, prob)
+    _assert_bit_exact(got, ref)
+    assert np.array_equal(got["mask"], ref["mask"])
 
 
 def test_rerun_on_resident_inputs_is_reproducible():

@@ -1,5 +1,6 @@
-"""Timing of the PatchMatch run under sets of environment knobs (B200PM_*): per-pass times for each configuration.
-usage: pm_time.py W H N "K1=V1 K2=V2" "K1=V3" ...   (each quoted argument is one configuration)"""
+"""Timing of the PatchMatch run, split into the rand(+msg) / pixel / serial passes, under sets of environment settings
+(the B200PM_WPC / B200PM_PRUNE / B200PM_PRUNE_FROM schedule seams): one line per configuration.
+usage: pm_time.py W H N "K1=V1 K2=V2" "K1=V3" ...   (each quoted argument is one configuration; none: the defaults)"""
 import os
 import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
