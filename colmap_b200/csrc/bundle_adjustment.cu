@@ -269,6 +269,7 @@ struct BaDev {
   const int2* c_pack;                 // [nobs_c] {point index, variable point index or -1} in camera order
   const int2* runs_pc;                // per run {pose index, camera index}
   int intr_by_pt;                     // some track sees one variable-intrinsics camera twice: intrinsics blocks via ba_schur_pt_kernel
+  int pose_by_pt;                     // some track sees one variable frame twice (rig sensors): pose blocks via ba_schur_pt_kernel too
   const int* c_run;                   // [nobs_c padded] run id of the observation in camera order: one run = one (camera, pose) pair
   const int4* runs;                   // per run {pose offset or -1, camera offset or -1, #variable intrinsics, 0}
   const int4* chunks;                 // {c0, c1, out offset, comp0 | ncomp << 8}: <= BA_CHUNK observations of one block
@@ -836,14 +837,14 @@ __global__ void __launch_bounds__(BA_SC_BLOCK) ba_cam_offdiag_kernel(const BaDev
 // reduced with shuffles, one red.add per entry per chunk.  Nothing per observation is written.  When a track sees the
 // same variable-intrinsics camera twice (shared cameras) the intrinsics blocks also need the cross terms between
 // different observations of the point: those problems set D.intr_by_pt and the intrinsics blocks come from
-// ba_schur_pt_kernel instead.
+// ba_schur_pt_kernel instead.  So do the pose blocks when a track sees a rig frame through two sensors (D.pose_by_pt).
 __global__ void __launch_bounds__(BA_SC_BLOCK) ba_schur_cam_kernel(const BaDev D) {
   const int chunk = blockIdx.x * (BA_SC_BLOCK / 32) + (threadIdx.x >> 5);
   if (chunk >= D.nchunks) return;
   const int lane = threadIdx.x & 31;
   const int4 ch = D.chunks[chunk];
   const int comp0 = ch.w & 0xff, n = (ch.w >> 8) & 0xff, lr0 = (ch.w >> 16) & 0xff, bw = (ch.w >> 24) & 0xff;
-  const bool want_T = (comp0 == 0) || !D.intr_by_pt;
+  const bool want_T = (comp0 == 0) ? !D.pose_by_pt : !D.intr_by_pt;
   double g[6] = {0, 0, 0, 0, 0, 0}, T[21];
 #pragma unroll
   for (int i = 0; i < 21; ++i) T[i] = 0.0;
@@ -956,13 +957,40 @@ __global__ void ba_damp_cam_kernel(const BaDev D, double inv_radius, double dmin
 // per point: the point term of the INTRINSICS blocks of SCHUR_JACOBI, -= V^T Hinv V with V summed over every
 // observation of the track made with the same camera (exact cross terms for shared intrinsics).  Only launched when
 // some track sees a variable-intrinsics camera more than once (D.intr_by_pt); otherwise ba_schur_cam_kernel has them.
+// When a track sees a frame through several rig sensors (D.pose_by_pt) the POSE blocks get the same treatment:
+// ceres' block of that frame holds the cross terms between those observations.
 __global__ void ba_schur_pt_kernel(const BaDev D) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= D.nvpt) return;
   const double* I = D.Hpp_inv + 6 * (long long)k;
   const double Hi[9] = {I[0], I[1], I[2], I[1], I[3], I[4], I[2], I[4], I[5]};
   const int s0 = D.vpt_s0[k], s1 = D.vpt_s1[k];
-  for (int s = s0; s < s1; ++s) {
+  if (D.pose_by_pt) for (int s = s0; s < s1; ++s) {
+    const int pi = D.s_pose[s], po = D.pose_off[pi];
+    if (po < 0) continue;
+    bool first = true;
+    for (int s2 = s0; s2 < s && first; ++s2) if (D.s_pose[s2] == pi) first = false;
+    if (!first) continue;
+    double V[18];
+    for (int t = 0; t < 18; ++t) V[t] = 0.0;
+    for (int s2 = s; s2 < s1; ++s2) {
+      if (D.s_pose[s2] != pi) continue;
+      double a2[3], b2[3];
+      for (int c = 0; c < 3; ++c) { a2[c] = D.Jp[BA_JP(c, s2)]; b2[c] = D.Jp[BA_JP(3 + c, s2)]; }
+      for (int c = 0; c < 6; ++c) {
+        const double j0 = D.Jc[BA_JC(c, s2)], j1 = D.Jc[BA_JC(D.DC + c, s2)];
+        for (int t = 0; t < 3; ++t) V[t * 6 + c] += a2[t] * j0 + b2[t] * j1;
+      }
+    }
+    double* M = D.Mbb + D.blk_pack[D.off2blk[po]];
+    for (int r = 0; r < 6; ++r) {
+      const double t0 = V[r] * Hi[0] + V[6 + r] * Hi[3] + V[12 + r] * Hi[6];
+      const double t1 = V[r] * Hi[1] + V[6 + r] * Hi[4] + V[12 + r] * Hi[7];
+      const double t2 = V[r] * Hi[2] + V[6 + r] * Hi[5] + V[12 + r] * Hi[8];
+      for (int c = 0; c < 6; ++c) atomicAdd(&M[r * 6 + c], -(t0 * V[c] + t1 * V[6 + c] + t2 * V[12 + c]));
+    }
+  }
+  if (D.intr_by_pt) for (int s = s0; s < s1; ++s) {
     const int ci = D.s_cam[s];
     const int co = D.cam_off[ci], nv = D.cam_width[ci];
     if (co < 0) continue;
@@ -1304,7 +1332,7 @@ __global__ void __launch_bounds__(BA_BLOCK) ba_cam_stream_loop_kernel(const BaDe
 
 // ---- PCG vector work between two SpMVs in one single-CTA kernel (camera-side dimension is small: a few thousand) ----
 #define BA_PCG_T 1024
-#define BA_PCG_FUSED_MAX 65536
+#define BA_PCG_FUSED_MAX 65536   // tests/test_ba_paths_gpu.py mirrors this threshold
 __device__ __forceinline__ double ba_cta_allsum(double v, double* sm /* [33] */) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
@@ -1323,7 +1351,8 @@ __device__ __forceinline__ double ba_cta_allsum(double v, double* sm /* [33] */)
 // One launch between two SpMVs: the tail of PCG iteration i (pq = p.q ; x += alpha p ; r -= alpha q ; Q1 = -x.(b + r) ;
 // |r|^2 ; termination, see ba_pcg_step_kernel) followed by the head of iteration i + 1 (z = M^-1 r ; rho = r.z ;
 // p = z + beta p ; q = D_c^2 p — the SpMV adds the rest).  do_post = 0 for the very first call of a solve.
-#define BA_PCG_EPT 4   // elements per thread handled from registers (nc <= BA_PCG_T * BA_PCG_EPT takes the fast path)
+#define BA_PCG_EPT 4   // elements per thread handled from registers (nc <= BA_PCG_T * BA_PCG_EPT takes the fast path;
+                      // tests/test_ba_paths_gpu.py mirrors this threshold)
 __global__ void __launch_bounds__(BA_PCG_T) ba_pcg_mid_kernel(const BaDev D, double q_tolerance, double r_tolerance,
                                                               int max_iters, int zero_q, int do_post, int r_in_smem) {
   extern __shared__ double s_r[];   // [nc] when r_in_smem
@@ -1436,12 +1465,12 @@ __global__ void __launch_bounds__(BA_PCG_T) ba_pcg_mid_kernel(const BaDev D, dou
   if (threadIdx.x == 0) c->rho = rho;
 }
 
-// Latency-tuned form of ba_pcg_mid_kernel for camera sides of up to BA_PCG_T * BA_MID_EPT unknowns (B3: 4993).  The
+// Latency-tuned form of ba_pcg_mid_kernel for camera sides of up to BA_PCG_T * BA_MID_EPT unknowns (B3: 3994).  The
 // single CTA is a chain of dependent memory round trips, so everything a thread will need is requested up front:
 // r, x, b and the block-row descriptors stream into shared memory with cp.async while p, q arrive in registers and the
 // first reduction runs; the rows of M^-1 are fetched with batched predicated loads.  Same arithmetic, in the same
 // order, as ba_pcg_mid_kernel (bit-identical results).
-#define BA_MID_EPT 5
+#define BA_MID_EPT 5   // tests/test_ba_paths_gpu.py mirrors the threshold BA_PCG_T * BA_MID_EPT
 #define BA_MID_STAGE_BYTES_PER_ROW 40   // r, x, b (doubles) + row_info (int4)
 __global__ void __launch_bounds__(BA_PCG_T) ba_pcg_mid_staged_kernel(const BaDev D, double q_tolerance, double r_tolerance,
                                                                      int max_iters, int zero_q, int do_post) {
@@ -1740,7 +1769,7 @@ __global__ void __launch_bounds__(BA_BLOCK) ba_dense_schur_kernel(const BaDev D)
 // tools/ba_small.py compares the two: the mapper's small reduced systems (nc = 64-80) are faster dense than by PCG to
 // 1e-12, while at nc = 450 (50 images, 80k observations) the dense build's 41M fp64 atomics per LM iteration lose - so
 // dense only below 256
-#define BA_DENSE_MAX 256
+#define BA_DENSE_MAX 256   // tests/test_ba_paths_gpu.py mirrors this threshold
 __global__ void __launch_bounds__(BA_DENSE_T) ba_dense_solve_kernel(const BaDev D) {
   __shared__ double s_d;
   __shared__ int s_bad;
@@ -2036,9 +2065,9 @@ struct BaStreamGuard {
   }
 };
 
-static int g_ba_spmv_smem = 1;  // pass 1 with p staged in shared memory when it fits (B200BA_SPMV_SMEM=0 disables)
+static int g_ba_spmv_smem = 1;  // pass 1 with p staged in shared memory when it fits (B200BA_SPMV_SMEM=0 disables; read by every solve)
 static int g_ba_sms = 0;
-#define BA_SPMV_SMEM_MAX (72 * 1024)
+#define BA_SPMV_SMEM_MAX (72 * 1024)   // tests/test_ba_paths_gpu.py mirrors this threshold
 template <int DC>
 static void ba_launch_spmv(const BaDev& D, cudaStream_t s) {
   if (D.nblocks_warp) {
@@ -2815,6 +2844,17 @@ static int ba_solve_impl(const b200ba_options* o, b200ba_problem* p, b200ba_summ
     std::vector<long long> cur(vcount.begin(), vcount.end() - 1);
     for (long long i = 0; i < NOBS; ++i) { const int pv = pt_var[p->obs_point_idx[i]]; if (pv >= 0) vobs[cur[pv]++] = i; }
   }
+  // rig sensors: a track that sees one variable frame twice (through two of its sensors) needs the cross terms between
+  // those observations in the frame's SCHUR_JACOBI block, which ba_schur_pt_kernel forms
+  int pose_by_pt = 0;
+  if (NS > 0) {
+    for (int k = 0; k < nvpt && !pose_by_pt; ++k)
+      for (long long a = vcount[k]; a < vcount[k + 1] && !pose_by_pt; ++a) {
+        const int pa = p->obs_pose_idx[vobs[a]];
+        if (pose_off[pa] < 0) continue;
+        for (long long b = a + 1; b < vcount[k + 1]; ++b) if (p->obs_pose_idx[vobs[b]] == pa) { pose_by_pt = 1; break; }
+      }
+  }
   tick("group observations by point");
   // pack whole tracks into blocks of BA_BLOCK slots.  The host only decides WHICH observation sits in which slot
   // (s_obs); every per-slot / per-camera-order array is then built on the device from the caller's raw arrays.
@@ -3073,6 +3113,7 @@ static int ba_solve_impl(const b200ba_options* o, b200ba_problem* p, b200ba_summ
   BA_CUDA(pool.alloc(&D.JcC, (size_t)2 * D.DC * nobs_c_pad)); BA_CUDA(pool.alloc(&D.u, (size_t)nobs_c_pad)); BA_CUDA(pool.alloc(&D.rC, (size_t)2 * nobs_c_pad)); BA_CUDA(pool.alloc(&D.JpC, (size_t)6 * nobs_c_pad));
   { int2* t; BA_CUDA(pool.upload(&t, runs_pc, st)); D.runs_pc = t; }
   D.intr_by_pt = intr_by_pt;
+  D.pose_by_pt = pose_by_pt;
   D.nblocks_warp = nblocks_warp; D.nblocks_giant0 = nblocks_giant0; D.nblocks_giant1 = nblocks_giant1;
   BA_CUDA(pool.alloc(&D.zg, (size_t)3 * nvpt));
   { int4* t; BA_CUDA(pool.upload(&t, chunks, st)); D.chunks = t; }
@@ -3166,11 +3207,12 @@ static int ba_solve_impl(const b200ba_options* o, b200ba_problem* p, b200ba_summ
   bool finished = false;
   const bool verbose = getenv("B200BA_VERBOSE") != nullptr;
   const bool fused_pcg = nc <= BA_PCG_FUSED_MAX && getenv("B200BA_PCG_MULTI") == nullptr;
+  // r of ba_pcg_mid_kernel in (at most 160 KB of) shared memory; tests/test_ba_paths_gpu.py mirrors this threshold
   const size_t mid_smem = (fused_pcg && (size_t)nc * sizeof(double) <= 160 * 1024 && getenv("B200BA_MID_GLOBAL") == nullptr) ? (size_t)nc * sizeof(double) : 0;
   if (mid_smem) BA_CUDA(cudaFuncSetAttribute(ba_pcg_mid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
   const size_t mid_staged = (fused_pcg && nc <= BA_PCG_T * BA_MID_EPT && getenv("B200BA_MID_PLAIN") == nullptr) ? (size_t)nc * BA_MID_STAGE_BYTES_PER_ROW : 0;
   if (mid_staged) BA_CUDA(cudaFuncSetAttribute(ba_pcg_mid_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_PCG_T * BA_MID_EPT * BA_MID_STAGE_BYTES_PER_ROW));
-  if (const char* e = getenv("B200BA_SPMV_SMEM")) g_ba_spmv_smem = atoi(e) != 0;
+  { const char* e = getenv("B200BA_SPMV_SMEM"); g_ba_spmv_smem = e ? atoi(e) != 0 : 1; }   // per solve: an unset variable restores the default
   double last_gmax = 0.0;
   int discarded_pcg = 0;
   while (!finished) {
@@ -3216,8 +3258,9 @@ static int ba_solve_impl(const b200ba_options* o, b200ba_problem* p, b200ba_summ
       if (nvpt && nc) {
         if (D.nchunks) ba_schur_cam_kernel<<<(D.nchunks + BA_SC_BLOCK / 32 - 1) / (BA_SC_BLOCK / 32), BA_SC_BLOCK, 0, st>>>(D);
         if (D.nchunks_off && !intr_by_pt) ba_cam_offdiag_kernel<true><<<(D.nchunks_off + BA_SC_BLOCK / 32 - 1) / (BA_SC_BLOCK / 32), BA_SC_BLOCK, 0, st>>>(D);
-        if (dkmax > 0 && intr_by_pt) ba_schur_pt_kernel<<<gp_blocks, 256, 0, st>>>(D);
-        launches += 1 + (dkmax > 0 && intr_by_pt ? 1 : 0);
+        const bool schur_pt = (dkmax > 0 && intr_by_pt) || D.pose_by_pt;
+        if (schur_pt) ba_schur_pt_kernel<<<gp_blocks, 256, 0, st>>>(D);
+        launches += 1 + (schur_pt ? 1 : 0);
       }
       mark(PF_DAMP_SCHUR);
       group_begin();

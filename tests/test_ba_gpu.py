@@ -273,10 +273,11 @@ from colmap_b200.bundle_adjustment import (DIVISION, EQUIRECTANGULAR, EUCM, FISH
     ((FULL_OPENCV,), True, dict(refine_principal_point=True)),                  # 12-wide block: two 6-ranges + their pair
     ((RAD_TAN_THIN_PRISM_FISHEYE,), True, dict(refine_principal_point=True)),   # 16-wide block
     ((FOV, EUCM, DIVISION, SIMPLE_DIVISION), False, {}),
-    ((SIMPLE_FISHEYE, THIN_PRISM_FISHEYE), True, dict(linear_solver_type=ITERATIVE_SCHUR)),
+    ((THIN_PRISM_FISHEYE,), True, dict(linear_solver_type=ITERATIVE_SCHUR)),    # a shared camera is of models[0] only
     ((EQUIRECTANGULAR, PINHOLE), False, {}),                                    # metadata parameters are never refined
     ((OPENCV_FISHEYE, FULL_OPENCV), False, dict(linear_solver_type=ITERATIVE_SCHUR)),   # own wide cameras, PCG: SCHUR_JACOBI blocks
                                                                                         # of 6 and 10 columns from the 6-range pairs
+    ((SIMPLE_FISHEYE,), True, dict(linear_solver_type=ITERATIVE_SCHUR)),
 ])
 def test_wide_model_grid_parity(models, shared, kw):
     """models_jacobian.h:322-1565 on the solve path: every model beyond the <= 5-parameter family through the wide kernel
