@@ -2036,8 +2036,9 @@ static int ba_fail(int code, const std::string& msg) { g_ba_error = msg; return 
 #define BA_CUDA(call)                                                                               \
   do {                                                                                              \
     cudaError_t e__ = (call);                                                                       \
-    if (e__ != cudaSuccess) { pool.release(); return ba_fail(-100, std::string(#call) + ": " + cudaGetErrorString(e__)); } \
+    if (e__ != cudaSuccess) return ba_fail(-100, std::string(#call) + ": " + cudaGetErrorString(e__)); \
   } while (0)
+#define BA_TRY(call) do { const int rc__ = (call); if (rc__) return rc__; } while (0)   // propagates a b200ba error code
 
 struct BaPool {
   std::vector<std::pair<void*, size_t>> ptrs;
@@ -2052,33 +2053,33 @@ struct BaPool {
     if (e != cudaSuccess) return e;
     return cudaMemcpyAsync(*p, v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice, s);
   }
+  template <typename T> cudaError_t upload(const T** p, const std::vector<T>& v, cudaStream_t s) {   // read-only BaDev fields
+    return upload(const_cast<T**>(p), v, s);
+  }
   void release() { if (ptrs.empty()) return; cudaDeviceSynchronize(); for (auto& a : ptrs) B200DeviceCache::get().free(a.first, a.second); ptrs.clear(); }
   ~BaPool() { release(); }   // every return path of a solve gives its blocks back
 };
-// stream + events of one solve: destroyed on every return path (declared after the pool, so before its release)
-struct BaStreamGuard {
-  cudaStream_t st = nullptr;
-  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-  ~BaStreamGuard() {
-    for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
-    if (st) { cudaStreamSynchronize(st); cudaStreamDestroy(st); }
-  }
-};
 
-static int g_ba_spmv_smem = 1;  // pass 1 with p staged in shared memory when it fits (B200BA_SPMV_SMEM=0 disables; read by every solve)
-static int g_ba_sms = 0;
+static int ba_sm_count() { int dev = 0, n = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); return n; }
+// The reduced-system kernels of one solve, chosen once per solve by ba_select_path from nc and the solver type.
+// B200BA_NO_DENSE, B200BA_PCG_MULTI, B200BA_MID_GLOBAL, B200BA_MID_PLAIN and B200BA_SPMV_SMEM=0 turn a path off (test seams).
+struct BaPath {
+  bool dense;          // dense Cholesky of the explicit reduced camera matrix
+  bool fused_pcg;      // single-CTA PCG vector step between the SpMVs (else five kernels per iteration)
+  bool spmv_smem;      // SpMV pass 1 of the warp-packed blocks with p staged in shared memory
+  size_t mid_smem;     // dynamic shared memory of ba_pcg_mid_kernel (> 0: r in shared memory)
+  size_t mid_staged;   // dynamic shared memory of ba_pcg_mid_staged_kernel (> 0: it runs instead of ba_pcg_mid_kernel)
+  int max_cg, sms;
+  double r_tol;        // relative residual that ends an exact PCG solve; -1 for ITERATIVE_SCHUR
+};
 #define BA_SPMV_SMEM_MAX (72 * 1024)   // tests/test_ba_paths_gpu.py mirrors this threshold
 template <int DC>
-static void ba_launch_spmv(const BaDev& D, cudaStream_t s) {
+static void ba_launch_spmv(const BaDev& D, const BaPath& P, cudaStream_t s) {
   if (D.nblocks_warp) {
     const size_t smem = sizeof(double) * (size_t)D.nc;
-    if (g_ba_spmv_smem && smem <= BA_SPMV_SMEM_MAX) {
-      // function attributes are per device: set on every launch that needs more than the default 48 KB (a process may
-      // drive several GPUs)
-      if (smem > 48 * 1024) cudaFuncSetAttribute(ba_schur_spmv_warp_smem_kernel<DC>, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_SPMV_SMEM_MAX);
-      if (!g_ba_sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&g_ba_sms, cudaDevAttrMultiProcessorCount, dev); }
+    if (P.spmv_smem) {
       const int per_sm = (int)std::max<size_t>(1, std::min<size_t>(5, (size_t)(216 * 1024) / (smem + 1024)));
-      const int grid = std::min(D.nblocks_warp, g_ba_sms * per_sm);
+      const int grid = std::min(D.nblocks_warp, P.sms * per_sm);
       ba_schur_spmv_warp_smem_kernel<DC><<<grid, BA_BLOCK, smem, s>>>(D, D.p);
     } else {
       ba_schur_spmv_warp_kernel<DC><<<D.nblocks_warp, BA_BLOCK, 0, s>>>(D, D.p);
@@ -2091,9 +2092,8 @@ static void ba_launch_spmv(const BaDev& D, cudaStream_t s) {
     ba_giant_finish_kernel<0><<<D.nblocks_giant1 - D.nblocks_giant0, BA_BLOCK, 0, s>>>(D, D.p);
   }
   if (D.nobs_c) {
-    if (!g_ba_sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&g_ba_sms, cudaDevAttrMultiProcessorCount, dev); }
     const long long ntiles = (D.nobs_c + 31) / 32;
-    const long long warps = (long long)g_ba_sms * 2 * (BA_BLOCK / 32) * 2;   // two waves of two resident CTAs per SM
+    const long long warps = (long long)P.sms * 2 * (BA_BLOCK / 32) * 2;   // two waves of two resident CTAs per SM
     const int tpw = (int)std::max<long long>(4, (ntiles + warps - 1) / warps);
     const unsigned grid = (unsigned)((ntiles + (long long)tpw * (BA_BLOCK / 32) - 1) / ((long long)tpw * (BA_BLOCK / 32)));
     ba_cam_stream_loop_kernel<DC><<<grid, BA_BLOCK, 0, s>>>(D, D.q, 1, tpw);
@@ -2116,39 +2116,26 @@ static void ba_launch_backsub(const BaDev& D, cudaStream_t s) {
     ba_giant_finish_kernel<1><<<D.nblocks_giant1 - D.nblocks_giant0, BA_BLOCK, 0, s>>>(D, D.x);
   }
 }
-template <int DC, bool WIDE>
-static void ba_launch_linearize_dc(const BaDev& D, int apply_scale, cudaStream_t s) {
+// DC = 6 + widest camera block.  6..11: the narrow layout (trivial frames, <= 5-parameter models); 14 / 18 / 22 / 28: the wide
+// instantiations (any model, rig sensors), DC rounded up to the next of them.
+template <int DC>
+static void ba_launch_linearize(const BaDev& D, int apply_scale, cudaStream_t s) {
+  constexpr bool WIDE = DC >= 14;
   ba_linearize_slot_kernel<DC, WIDE><<<D.nblocks, BA_BLOCK, 0, s>>>(D, apply_scale, &D.ctl->cost);
   if (D.nobs_c) ba_linearize_cam_kernel<DC, WIDE><<<(unsigned)((D.nobs_c + BA_BLOCK - 1) / BA_BLOCK), BA_BLOCK, 0, s>>>(D, apply_scale);
 }
-// DC = 6 + widest camera block.  6..11: the narrow layout (trivial frames, <= 5-parameter models); 14 / 18 / 22 / 28: the wide
-// instantiations (any model, rig sensors), DC rounded up to the next of them.
-static void ba_launch_linearize(const BaDev& D, int apply_scale, cudaStream_t s) {
-  switch (D.DC) {
-    case 6: ba_launch_linearize_dc<6, false>(D, apply_scale, s); break;
-    case 7: ba_launch_linearize_dc<7, false>(D, apply_scale, s); break;
-    case 8: ba_launch_linearize_dc<8, false>(D, apply_scale, s); break;
-    case 9: ba_launch_linearize_dc<9, false>(D, apply_scale, s); break;
-    case 10: ba_launch_linearize_dc<10, false>(D, apply_scale, s); break;
-    case 11: ba_launch_linearize_dc<11, false>(D, apply_scale, s); break;
-    case 14: ba_launch_linearize_dc<14, true>(D, apply_scale, s); break;
-    case 18: ba_launch_linearize_dc<18, true>(D, apply_scale, s); break;
-    case 22: ba_launch_linearize_dc<22, true>(D, apply_scale, s); break;
-    default: ba_launch_linearize_dc<28, true>(D, apply_scale, s); break;
-  }
-}
-#define BA_DISPATCH_DC(FN, D, s)                 \
+#define BA_DISPATCH_DC(FN, D, ...)               \
   switch ((D).DC) {                              \
-    case 6: FN<6>(D, s); break;                  \
-    case 7: FN<7>(D, s); break;                  \
-    case 8: FN<8>(D, s); break;                  \
-    case 9: FN<9>(D, s); break;                  \
-    case 10: FN<10>(D, s); break;                \
-    case 11: FN<11>(D, s); break;                \
-    case 14: FN<14>(D, s); break;                \
-    case 18: FN<18>(D, s); break;                \
-    case 22: FN<22>(D, s); break;                \
-    default: FN<28>(D, s); break;                \
+    case 6: FN<6>(D, __VA_ARGS__); break;        \
+    case 7: FN<7>(D, __VA_ARGS__); break;        \
+    case 8: FN<8>(D, __VA_ARGS__); break;        \
+    case 9: FN<9>(D, __VA_ARGS__); break;        \
+    case 10: FN<10>(D, __VA_ARGS__); break;      \
+    case 11: FN<11>(D, __VA_ARGS__); break;      \
+    case 14: FN<14>(D, __VA_ARGS__); break;      \
+    case 18: FN<18>(D, __VA_ARGS__); break;      \
+    case 22: FN<22>(D, __VA_ARGS__); break;      \
+    default: FN<28>(D, __VA_ARGS__); break;      \
   }
 
 
@@ -2323,6 +2310,69 @@ static void ba_p2p_ensure(b200ba_comm* c, size_t need_doubles, cudaStream_t st) 
   if (!opened) { ba_p2p_teardown(c); P.tried = true; return; }
   P.cap = cap; P.bytes = bytes; P.ok = true;
 }
+
+// All-reduce of device buffers over the ranks of a sharded solve (no-op without a communicator).  Calls between begin()
+// and end() travel together: as ONE launch of the peer-memory kernel when the communicator has its symmetric buffers
+// mapped (ba_p2p_ensure) and the payload is latency-sized, else as one NCCL group.
+struct BaReducer {
+  struct Red { void* buf; size_t count; ncclDataType_t dt; ncclRedOp_t op; const int* done; };
+  b200ba_comm* comm = nullptr;   // set only for a sharded solve (world > 1)
+  cudaStream_t st = nullptr;
+  BaPool* pool = nullptr;        // holds the device copies of agree()
+  int sms = 0, launches = 0;     // launches of ba_p2p_allreduce_kernel
+  bool grouped = false;
+  std::vector<Red> pending;
+  cudaError_t operator()(void* buf, size_t count, ncclDataType_t dt, ncclRedOp_t op, const int* done = nullptr) {
+    if (!comm || count == 0) return cudaSuccess;
+    pending.push_back({buf, count, dt, op, done});
+    return grouped ? cudaSuccess : flush();
+  }
+  void begin() { grouped = true; }
+  cudaError_t end() { grouped = false; return flush(); }
+  // the host vector v becomes the reduction of every rank's v
+  template <typename T> int agree(std::vector<T>& v, ncclDataType_t dt, ncclRedOp_t op) {
+    T* d;
+    BA_CUDA(pool->upload(&d, v, st));
+    BA_CUDA((*this)(d, v.size(), dt, op));
+    BA_CUDA(cudaMemcpyAsync(v.data(), d, sizeof(T) * v.size(), cudaMemcpyDeviceToHost, st));
+    BA_CUDA(cudaStreamSynchronize(st));
+    return 0;
+  }
+  cudaError_t flush() {
+    if (pending.empty()) return cudaSuccess;
+    size_t total = 0;
+    bool p2p = comm->p2p.ok && pending.size() <= 3;
+    for (const Red& r : pending) {
+      total += r.count;
+      const bool f64 = r.dt == ncclDouble && (r.op == ncclSum || r.op == ncclMax), i32 = r.dt == ncclInt32 && r.op == ncclMax;
+      if (!f64 && !i32) p2p = false;
+    }
+    if (p2p && (total > comm->p2p.cap || total * sizeof(double) > BA_P2P_MAX_BYTES)) p2p = false;
+    if (p2p) {
+      BaP2PArgs A;
+      memset(&A, 0, sizeof(A));
+      for (size_t i = 0; i < pending.size(); ++i) {
+        const Red& r = pending[i];
+        A.seg[i].ptr = r.buf; A.seg[i].count = (int)r.count;
+        A.seg[i].kind = r.dt == ncclInt32 ? BA_RED_I32_MAX : (r.op == ncclSum ? BA_RED_F64_SUM : BA_RED_F64_MAX);
+      }
+      A.nseg = (int)pending.size(); A.total = (int)total; A.rank = comm->rank; A.world = comm->world; A.cap = comm->p2p.cap;
+      for (int r = 0; r < comm->world; ++r) A.peer[r] = comm->p2p.peer[r];
+      A.state = comm->p2p.state; A.done = pending[0].done;
+      const int ctas = (int)std::min<size_t>(2 * (size_t)sms, std::max<size_t>(1, (total + 255) / 256));   // all CTAs resident: they wait for each other's peers
+      ba_p2p_allreduce_kernel<<<ctas, 256, 0, st>>>(A);
+      ++launches;
+      pending.clear();
+      return cudaGetLastError();
+    }
+    ncclResult_t res = ncclSuccess;
+    if (pending.size() > 1) ba_nccl().GroupStart();
+    for (const Red& r : pending) { const ncclResult_t q = ba_nccl().AllReduce(r.buf, r.buf, r.count, r.dt, r.op, comm->comm, st); if (q != ncclSuccess) res = q; }
+    if (pending.size() > 1) ba_nccl().GroupEnd();
+    pending.clear();
+    return res == ncclSuccess ? cudaSuccess : cudaErrorUnknown;
+  }
+};
 
 static int ba_solve_impl(const b200ba_options* o, b200ba_problem* p, b200ba_summary* sum, b200ba_comm* comm);
 
@@ -2641,725 +2691,725 @@ void b200ba_comm_destroy(b200ba_comm_t c) {
 
 }  // extern "C"
 
-// Host-side slot layout handed to the CPU test tier (b200ba_test_pack): filled when set and the solve runs host-only.
-struct BaHostLayout {
-  std::vector<int> s_obs, s_lpt, s_seg, vpt_s0, vpt_s1, vpt_point;
-  int nblocks_warp = 0, nblocks_var = 0, nblocks_giant0 = 0, nblocks_giant1 = 0, nc = 0, nvpt = 0, dkmax = 0;
-  int num_residuals = 0, num_effective_parameters = 0;
+// ---- host flattening: everything a solve decides before the device is involved ----
+// The slot layout packs whole tracks into blocks of BA_BLOCK slots.  The host only decides WHICH observation sits in
+// which slot (s_obs); every per-slot / per-camera-order array is built on the device from the caller's arrays.
+struct BaLayout {
+  bool wide = false;                 // any camera model beyond the <= 5-parameter family, or any rig sensor
+  bool nothing_to_solve = false;     // no effective observation or no effective parameter
+  int lst = 0;                       // linear solver type, AUTO resolved
+  std::vector<int> pose_off, cam_off, cam_nvar, cam_poff, cam_model, pt_var, cam_sensor, cam_ns, cam_width, sens_cam;
+  std::vector<unsigned char> pose_mask;
+  std::vector<signed char> cam_var;  // [ncams * BA_MAXP] indices of the variable intrinsics
+  std::vector<int> blk_start, blk_pack, blk_split, off2blk;                        // camera-side blocks
+  std::vector<int> s_obs, s_lpt, s_seg, blk_pt0, blk_npt, vpt_s0, vpt_s1, vpt_point;  // slots, variable points
+  int nc = 0, nblk = 0, pack = 0, dkmax = 0, DC = 6, nvpt = 0, pose_by_pt = 0;
+  int nblocks = 0, nblocks_warp = 0, nblocks_giant0 = 0, nblocks_giant1 = 0;
+  long long ncamparams = 0, nobs_eff = 0;   // nobs_eff: observations of this rank connected to a variable block
 };
-static thread_local BaHostLayout* g_ba_layout_out = nullptr;
 
-static int ba_solve_impl(const b200ba_options* o, b200ba_problem* p, b200ba_summary* sum, b200ba_comm* comm) {
-  if (!o || !p || !sum) return ba_fail(-1, "null argument");
-  memset(sum, 0, sizeof(*sum));
-  sum->termination_type = B200BA_FAILURE;
-  BaPool pool;
-  const auto t_setup0 = std::chrono::steady_clock::now();
-  const bool host_only = getenv("B200BA_HOST_ONLY") != nullptr || g_ba_layout_out != nullptr;   // diagnostic / CPU tests: stop after the host flattening
-  auto tick = [&](const char* what) { if (host_only && !g_ba_layout_out) fprintf(stderr, "[b200ba host] %-28s %8.1f ms\n", what, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_setup0).count()); };
-  int ndev = 0;
-  if (!host_only && (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)) return ba_fail(-101, "no CUDA device: colmap_b200 has no CPU fallback");
-  if (!host_only && o->gpu_index >= 0) {
-    if (o->gpu_index >= ndev) return ba_fail(-101, "gpu_index out of range");
-    cudaSetDevice(o->gpu_index);
-  }
-  // ---------------------------------------------------------------- flatten (host)
-  const int NP = p->num_poses, NCAM = p->num_cameras;
+// Validation, the "used" flags and the variable blocks: pose and camera offsets and masks, camera blocks, variable points.
+// neff_cam: effective camera-side parameters.
+static int ba_flatten_blocks(const b200ba_options* o, const b200ba_problem* p, BaReducer* red, BaLayout& L,
+                             std::vector<int>& used, int& neff_cam) {
+  const int NP = p->num_poses, NCAM = p->num_cameras, NS = p->num_sensors;
   const long long NPT = p->num_points, NOBS = p->num_observations;
   for (int c = 0; c < NCAM; ++c) if (ba_model_num_params(p->camera_model_id[c]) < 0) return ba_fail(-2, "unknown camera model id");
-  const int NS = p->num_sensors;
-  bool wide = NS > 0;
+  L.wide = NS > 0;
   for (int c = 0; c < NCAM; ++c) {
-    if (!ba_model_is_narrow(p->camera_model_id[c])) wide = true;
+    if (!ba_model_is_narrow(p->camera_model_id[c])) L.wide = true;
     if (p->camera_sensor_idx && p->camera_sensor_idx[c] >= NS) return ba_fail(-2, "camera_sensor_idx out of range");
   }
   if (NS > 0 && (!p->sensor_from_rig || !p->camera_sensor_idx)) return ba_fail(-2, "rig sensors need sensor_from_rig and camera_sensor_idx");
-  std::vector<unsigned char> pose_used(NP, 0), cam_used(NCAM, 0), pt_used(NPT, 0);
+  used.assign(NP + NCAM, 0);   // [poses | cameras]
+  std::vector<unsigned char> pt_used(NPT, 0);
   for (long long i = 0; i < NOBS; ++i) {   // range check and "block appears in an observation" in one pass
     const int a = p->obs_pose_idx[i], b = p->obs_camera_idx[i], c = p->obs_point_idx[i];
     if ((unsigned)a >= (unsigned)NP || (unsigned)b >= (unsigned)NCAM || c < 0 || c >= NPT) return ba_fail(-2, "observation index out of range");
-    pose_used[a] = 1; cam_used[b] = 1; pt_used[c] = 1;
+    used[a] = 1; used[NP + b] = 1; pt_used[c] = 1;
   }
-  const bool sharded = comm != nullptr && comm->world > 1;
-  BaStreamGuard guard;
-  if (!host_only) BA_CUDA(cudaStreamCreateWithFlags(&guard.st, cudaStreamNonBlocking));
-  const cudaStream_t st = guard.st;
-  // all-reduce of device buffers over the ranks of a sharded solve (no-op otherwise).  Calls between group_begin() and
-  // group_end() travel together: as ONE launch of the peer-memory kernel when the communicator has its symmetric
-  // buffers mapped (ba_p2p_ensure) and the payload is latency-sized, else as one NCCL group.
-  struct PendingRed { void* buf; size_t count; ncclDataType_t dt; ncclRedOp_t op; const int* done; };
-  std::vector<PendingRed> pending;
-  bool in_group = false;
-  int p2p_launches = 0, p2p_sms = 132;
-  if (sharded && !host_only) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&p2p_sms, cudaDevAttrMultiProcessorCount, dev); }
-  auto flush_reds = [&]() -> cudaError_t {
-    if (pending.empty()) return cudaSuccess;
-    size_t total = 0;
-    bool p2p = comm->p2p.ok && pending.size() <= 3;
-    for (const PendingRed& r : pending) {
-      total += r.count;
-      const bool f64 = r.dt == ncclDouble && (r.op == ncclSum || r.op == ncclMax), i32 = r.dt == ncclInt32 && r.op == ncclMax;
-      if (!f64 && !i32) p2p = false;
-    }
-    if (p2p && (total > comm->p2p.cap || total * sizeof(double) > BA_P2P_MAX_BYTES)) p2p = false;
-    if (p2p) {
-      BaP2PArgs A;
-      memset(&A, 0, sizeof(A));
-      for (size_t i = 0; i < pending.size(); ++i) {
-        const PendingRed& r = pending[i];
-        A.seg[i].ptr = r.buf; A.seg[i].count = (int)r.count;
-        A.seg[i].kind = r.dt == ncclInt32 ? BA_RED_I32_MAX : (r.op == ncclSum ? BA_RED_F64_SUM : BA_RED_F64_MAX);
-      }
-      A.nseg = (int)pending.size(); A.total = (int)total; A.rank = comm->rank; A.world = comm->world; A.cap = comm->p2p.cap;
-      for (int r = 0; r < comm->world; ++r) A.peer[r] = comm->p2p.peer[r];
-      A.state = comm->p2p.state; A.done = pending[0].done;
-      const int ctas = (int)std::min<size_t>(2 * (size_t)p2p_sms, std::max<size_t>(1, (total + 255) / 256));   // all CTAs resident: they wait for each other's peers
-      ba_p2p_allreduce_kernel<<<ctas, 256, 0, st>>>(A);
-      ++p2p_launches;
-      pending.clear();
-      return cudaGetLastError();
-    }
-    ncclResult_t res = ncclSuccess;
-    if (pending.size() > 1) ba_nccl().GroupStart();
-    for (const PendingRed& r : pending) { const ncclResult_t q = ba_nccl().AllReduce(r.buf, r.buf, r.count, r.dt, r.op, comm->comm, st); if (q != ncclSuccess) res = q; }
-    if (pending.size() > 1) ba_nccl().GroupEnd();
-    pending.clear();
-    return res == ncclSuccess ? cudaSuccess : cudaErrorUnknown;
-  };
-  auto allreduce_if = [&](void* buf, size_t count, ncclDataType_t dt, ncclRedOp_t op, const int* done) -> cudaError_t {
-    if (!sharded || count == 0) return cudaSuccess;
-    pending.push_back({buf, count, dt, op, done});
-    return in_group ? cudaSuccess : flush_reds();
-  };
-  auto allreduce = [&](void* buf, size_t count, ncclDataType_t dt, ncclRedOp_t op) -> cudaError_t { return allreduce_if(buf, count, dt, op, nullptr); };
-  auto group_begin = [&]() { in_group = true; };
-  auto group_end = [&]() -> cudaError_t { in_group = false; return sharded ? flush_reds() : cudaSuccess; };
-  if (sharded) {  // a block is "used" if any rank observes it: keeps the camera-side layout identical on every rank
-    std::vector<int> flags(NP + NCAM);
-    for (int i = 0; i < NP; ++i) flags[i] = pose_used[i];
-    for (int c = 0; c < NCAM; ++c) flags[NP + c] = cam_used[c];
-    int* d_flags;
-    BA_CUDA(pool.upload(&d_flags, flags, st));
-    BA_CUDA(allreduce(d_flags, flags.size(), ncclInt32, ncclMax));
-    BA_CUDA(cudaMemcpyAsync(flags.data(), d_flags, sizeof(int) * flags.size(), cudaMemcpyDeviceToHost, st));
-    BA_CUDA(cudaStreamSynchronize(st));
-    for (int i = 0; i < NP; ++i) pose_used[i] = (unsigned char)flags[i];
-    for (int c = 0; c < NCAM; ++c) cam_used[c] = (unsigned char)flags[NP + c];
-  }
-  tick("validate + used flags");
-  std::vector<int> pose_off(NP, -1), cam_off(NCAM, -1), cam_nvar(NCAM, 0), cam_poff(NCAM), cam_model(NCAM), pt_var(NPT, -1);
-  std::vector<unsigned char> pose_mask(NP, 0);
-  std::vector<signed char> cam_var(BA_MAXP * (size_t)NCAM, 0);
-  int off = 0, neff = 0, dkmax = 0;
-  std::vector<int> blk_start, blk_pack;
-  int pack = 0;
+  // sharded: a block is "used" if any rank observes it, which keeps the camera-side layout identical on every rank
+  if (red) BA_TRY(red->agree(used, ncclInt32, ncclMax));
+  const int* cam_used = used.data() + NP;
+  L.pose_off.assign(NP, -1); L.pose_mask.assign(NP, 0); L.cam_off.assign(NCAM, -1); L.cam_nvar.assign(NCAM, 0);
+  L.cam_poff.resize(NCAM); L.cam_model.resize(NCAM); L.pt_var.assign(NPT, -1); L.cam_var.assign(BA_MAXP * (size_t)NCAM, 0);
+  int off = 0, pack = 0;
+  neff_cam = 0;
   for (int i = 0; i < NP; ++i) {
-    const bool cst = !o->refine_rig_from_world || (p->pose_constant && p->pose_constant[i]) || !pose_used[i];
+    const bool cst = !o->refine_rig_from_world || (p->pose_constant && p->pose_constant[i]) || !used[i];
     if (cst) continue;
     unsigned m = 0x3f;
     if (o->constant_rig_from_world_rotation) m &= ~0x07u;
     if (p->pose_fixed_translation_dim && p->pose_fixed_translation_dim[i] >= 0) m &= ~(1u << (3 + p->pose_fixed_translation_dim[i]));
-    pose_off[i] = off; pose_mask[i] = (unsigned char)m; blk_start.push_back(off); blk_pack.push_back(pack); off += 6; pack += 36;
-    neff += __builtin_popcount(m);
+    L.pose_off[i] = off; L.pose_mask[i] = (unsigned char)m; L.blk_start.push_back(off); L.blk_pack.push_back(pack); off += 6; pack += 36;
+    neff_cam += __builtin_popcount(m);
   }
-  long long ncamparams = 0;
-  std::vector<int> cam_sensor(NCAM, -1), cam_ns(NCAM, 0), cam_width(NCAM, 0), sens_cam(NS, -1), blk_split;
-  blk_split.assign(blk_start.size(), 0);
+  L.cam_sensor.assign(NCAM, -1); L.cam_ns.assign(NCAM, 0); L.cam_width.assign(NCAM, 0); L.sens_cam.assign(NS, -1);
+  L.blk_split.assign(L.blk_start.size(), 0);
   for (int c = 0; c < NCAM; ++c) {
     const int id = p->camera_model_id[c], P = ba_model_num_params(id);
-    cam_model[c] = id; cam_poff[c] = p->camera_param_offset[c];
-    ncamparams = std::max<long long>(ncamparams, cam_poff[c] + P);
+    L.cam_model[c] = id; L.cam_poff[c] = p->camera_param_offset[c];
+    L.ncamparams = std::max<long long>(L.ncamparams, L.cam_poff[c] + P);
     int nv = 0;
     if (!(p->camera_constant && p->camera_constant[c]) && cam_used[c])
       for (int k = 0; k < P; ++k) {
         const int g = ba_param_group(id, k);
         const int refine = g == 0 ? o->refine_focal_length : (g == 1 ? o->refine_principal_point : (g == 2 ? o->refine_extra_params : 0));
-        if (refine) cam_var[BA_MAXP * (size_t)c + nv++] = (signed char)k;
+        if (refine) L.cam_var[BA_MAXP * (size_t)c + nv++] = (signed char)k;
       }
-    cam_nvar[c] = nv;
+    L.cam_nvar[c] = nv;
     // the camera's sensor_from_rig (non-reference rig sensor): variable iff refined, not constant and observed
     // (ParameterizeRigsAndFrames, bundle_adjustment_ceres.cc:478-539)
     const int si = (NS > 0) ? p->camera_sensor_idx[c] : -1;
-    cam_sensor[c] = si;
+    L.cam_sensor[c] = si;
     if (si >= 0) {
-      if (sens_cam[si] >= 0) return ba_fail(-2, "a sensor_from_rig pose must belong to exactly one camera");
-      sens_cam[si] = c;
-      if (o->refine_sensor_from_rig && !(p->sensor_constant && p->sensor_constant[si]) && cam_used[c]) cam_ns[c] = 6;
+      if (L.sens_cam[si] >= 0) return ba_fail(-2, "a sensor_from_rig pose must belong to exactly one camera");
+      L.sens_cam[si] = c;
+      if (o->refine_sensor_from_rig && !(p->sensor_constant && p->sensor_constant[si]) && cam_used[c]) L.cam_ns[c] = 6;
     }
-    const int w = cam_ns[c] + nv;
-    cam_width[c] = w;
+    const int w = L.cam_ns[c] + nv;
+    L.cam_width[c] = w;
     if (w) {
-      cam_off[c] = off; blk_start.push_back(off); blk_pack.push_back(pack); blk_split.push_back((cam_ns[c] && nv) ? 6 : 0);
-      off += w; pack += w * w; neff += w; dkmax = std::max(dkmax, w);
+      L.cam_off[c] = off; L.blk_start.push_back(off); L.blk_pack.push_back(pack); L.blk_split.push_back((L.cam_ns[c] && nv) ? 6 : 0);
+      off += w; pack += w * w; neff_cam += w; L.dkmax = std::max(L.dkmax, w);
     }
   }
-  const int nc = off, nblk = (int)blk_start.size();
-  blk_start.push_back(nc); blk_pack.push_back(pack);
-  std::vector<int> off2blk(nc);
-  for (int b = 0; b < nblk; ++b) for (int i = blk_start[b]; i < blk_start[b + 1]; ++i) off2blk[i] = b;
-  int nvpt = 0;
+  L.nc = off; L.nblk = (int)L.blk_start.size(); L.pack = pack;
+  L.blk_start.push_back(L.nc); L.blk_pack.push_back(pack);
+  L.off2blk.resize(L.nc);
+  for (int b = 0; b < L.nblk; ++b) for (int i = L.blk_start[b]; i < L.blk_start[b + 1]; ++i) L.off2blk[i] = b;
   for (long long i = 0; i < NPT; ++i) {
     const bool cst = !o->refine_points3D || (p->point_constant && p->point_constant[i]) || !pt_used[i];
-    if (!cst) pt_var[i] = nvpt++;
+    if (!cst) L.pt_var[i] = L.nvpt++;
   }
-  neff += 3 * nvpt;
+  return 0;
+}
+// Packs the tracks (observations vobs[vcount[k] .. vcount[k + 1]) of variable point k) into slots.  Variable points are
+// renumbered: tracks of <= 32 observations first (packed so that none crosses a warp), then the longer ones (packed so
+// that none crosses a block), then those longer than a block; the observations of constant points follow.
+static void ba_pack_tracks(const std::vector<long long>& vcount, const std::vector<long long>& vobs,
+                           const std::vector<long long>& const_obs, BaLayout& L) {
+  const int nvpt = L.nvpt;
+  const size_t cap = (size_t)(L.nobs_eff + L.nobs_eff / 8 + 4 * BA_BLOCK);
+  L.s_obs.reserve(cap); L.s_lpt.reserve(cap); L.s_seg.reserve(cap);
+  L.vpt_s0.resize(nvpt); L.vpt_s1.resize(nvpt); L.vpt_point.resize(nvpt);
+  std::vector<int> order_pts; order_pts.reserve(nvpt);
+  std::vector<long long> olen(nvpt), ostart(nvpt);
+  for (int k = 0; k < nvpt; ++k) { olen[k] = vcount[k + 1] - vcount[k]; ostart[k] = vcount[k]; }
+  {  // short tracks: fill every 32-slot warp greedily with the longest track that still fits (length buckets), so that
+     // almost no slot is padding (a first-come packing wastes ~11% at an average track length of 6-7)
+    std::vector<std::vector<int>> bucket(33);
+    for (int k = nvpt - 1; k >= 0; --k) if (olen[k] <= 32) bucket[olen[k]].push_back(k);   // pop_back yields ascending k
+    size_t remaining = 0;
+    for (int l = 1; l <= 32; ++l) remaining += bucket[l].size();
+    while (remaining) {
+      int cap = 32;
+      while (cap > 0) {
+        int l = std::min(cap, 32);
+        while (l > 0 && bucket[l].empty()) --l;
+        if (l == 0) break;
+        order_pts.push_back(bucket[l].back()); bucket[l].pop_back(); --remaining;
+        cap -= l;
+      }
+    }
+  }
+  const int nshort = (int)order_pts.size();
+  for (int k = 0; k < nvpt; ++k) if (olen[k] > 32 && olen[k] <= BA_BLOCK) order_pts.push_back(k);
+  const int nmid = (int)order_pts.size();
+  for (int k = 0; k < nvpt; ++k) if (olen[k] > BA_BLOCK) order_pts.push_back(k);
+  // renumber: new variable index = position in order_pts
+  std::vector<int> newidx(nvpt);
+  for (int n = 0; n < nvpt; ++n) newidx[order_pts[n]] = n;
+  for (int& v : L.pt_var) if (v >= 0) v = newidx[v];
+  for (size_t i = 0; i < L.pt_var.size(); ++i) if (L.pt_var[i] >= 0) L.vpt_point[L.pt_var[i]] = (int)i;
+  auto pad_to = [&](size_t mult) {
+    const size_t r = L.s_obs.size() % mult;
+    if (r) { const size_t add = mult - r; L.s_obs.insert(L.s_obs.end(), add, -1); L.s_lpt.insert(L.s_lpt.end(), add, -1); L.s_seg.insert(L.s_seg.end(), add, 0); }
+  };
+  auto append_track = [&](int n, int seg) {   // variable point n: its observations vobs[ostart .. ostart + olen)
+    const int k = order_pts[n];
+    const size_t at = L.s_obs.size(), len = (size_t)olen[k];
+    L.vpt_s0[n] = (int)at;
+    L.s_obs.resize(at + len); L.s_lpt.insert(L.s_lpt.end(), len, n); L.s_seg.insert(L.s_seg.end(), len, seg);
+    for (size_t j = 0; j < len; ++j) L.s_obs[at + j] = (int)vobs[ostart[k] + (long long)j];
+    L.vpt_s1[n] = (int)L.s_obs.size();
+  };
+  auto note_block = [&](int n) {
+    const int b = (int)(L.s_obs.size() / BA_BLOCK);
+    while ((int)L.blk_pt0.size() <= b) { L.blk_pt0.push_back(n); L.blk_npt.push_back(0); }
+    L.blk_npt[b]++;
+  };
+  for (int n = 0; n < nshort; ++n) {
+    const int len = (int)olen[order_pts[n]];
+    if ((int)(L.s_obs.size() % 32) + len > 32) pad_to(32);
+    note_block(n);
+    const int head = (int)(L.s_obs.size() % 32), last = head + len - 1;
+    append_track(n, head | (last << 8));
+  }
+  pad_to(BA_BLOCK);
+  L.nblocks_warp = (int)(L.s_obs.size() / BA_BLOCK);
+  for (int n = nshort; n < nmid; ++n) {
+    if ((int)(L.s_obs.size() % BA_BLOCK) + (int)olen[order_pts[n]] > BA_BLOCK) pad_to(BA_BLOCK);
+    note_block(n);
+    append_track(n, 0);
+  }
+  pad_to(BA_BLOCK);
+  L.nblocks_giant0 = (int)(L.s_obs.size() / BA_BLOCK);
+  for (int n = nmid; n < nvpt; ++n) append_track(n, 0);   // tracks longer than a block: back to back, generic kernels
+  pad_to(BA_BLOCK);
+  L.nblocks_giant1 = (int)(L.s_obs.size() / BA_BLOCK);
+  for (long long i : const_obs) { L.s_obs.push_back((int)i); L.s_lpt.push_back(-1); L.s_seg.push_back(0); }
+  pad_to(BA_BLOCK);
+  L.nblocks = (int)(L.s_obs.size() / BA_BLOCK);
+  L.blk_pt0.resize(L.nblocks, nvpt); L.blk_npt.resize(L.nblocks, 0);
+}
+// The host flattening of a solve.  red: the reducer of a sharded solve (the ranks agree on the used blocks and on the
+// counts), null for a single-GPU solve, which then touches no CUDA API.  Fills the sizes and the solver type of *sum.
+static int ba_flatten(const b200ba_options* o, const b200ba_problem* p, BaReducer* red, BaLayout& L, b200ba_summary* sum) {
+  const int NP = p->num_poses;
+  const long long NOBS = p->num_observations;
+  std::vector<int> used;   // poses, cameras
+  int neff = 0;
+  BA_TRY(ba_flatten_blocks(o, p, red, L, used, neff));
+  const int nvpt = L.nvpt;
   // effective observations grouped by variable point
-  std::vector<long long> vcount(nvpt + 1, 0);
-  std::vector<long long> const_obs;
-  long long nobs_eff = 0;
+  std::vector<long long> vcount(nvpt + 1, 0), const_obs;
   for (long long i = 0; i < NOBS; ++i) {
-    const int pv = pt_var[p->obs_point_idx[i]];
-    if (pv >= 0) { vcount[pv + 1]++; nobs_eff++; }
-    else if (pose_off[p->obs_pose_idx[i]] >= 0 || cam_off[p->obs_camera_idx[i]] >= 0) { const_obs.push_back(i); nobs_eff++; }
+    const int pv = L.pt_var[p->obs_point_idx[i]];
+    if (pv >= 0) { vcount[pv + 1]++; L.nobs_eff++; }
+    else if (L.pose_off[p->obs_pose_idx[i]] >= 0 || L.cam_off[p->obs_camera_idx[i]] >= 0) { const_obs.push_back(i); L.nobs_eff++; }
   }
-  long long g_nobs_eff = nobs_eff, g_pt_params = 3LL * nvpt;
-  if (sharded) {
-    std::vector<long long> cnt = {nobs_eff, 3LL * nvpt};
-    long long* d_cnt;
-    BA_CUDA(pool.upload(&d_cnt, cnt, st));
-    BA_CUDA(allreduce(d_cnt, 2, ncclInt64, ncclSum));
-    BA_CUDA(cudaMemcpyAsync(cnt.data(), d_cnt, 16, cudaMemcpyDeviceToHost, st));
-    BA_CUDA(cudaStreamSynchronize(st));
-    g_nobs_eff = cnt[0]; g_pt_params = cnt[1];
-  }
-  neff = neff - 3 * nvpt + (int)g_pt_params;
-  sum->num_residuals = (int)(2 * g_nobs_eff);
+  std::vector<long long> cnt = {L.nobs_eff, 3LL * nvpt};   // over all ranks: effective observations, point parameters
+  if (red) BA_TRY(red->agree(cnt, ncclInt64, ncclSum));
+  neff += (int)cnt[1];
+  sum->num_residuals = (int)(2 * cnt[0]);
   sum->num_effective_parameters = neff;
-  int lst = o->linear_solver_type;
-  if (lst == B200BA_AUTO) {
+  L.lst = o->linear_solver_type;
+  if (L.lst == B200BA_AUTO) {
     // config.NumImages() decides (bundle_adjustment_ceres.cc:131,204-210), not the number of poses of the whole model:
     // a local BA of six images inside a large reconstruction is a DENSE_SCHUR problem.  Flat callers that do not say
     // get the number of poses that appear in observations.
     int nimg = p->num_config_images;
-    if (nimg <= 0) for (int i = 0; i < NP; ++i) nimg += pose_used[i] ? 1 : 0;
-    lst = nimg <= 50 ? B200BA_DENSE_SCHUR : (nimg <= 1000 ? B200BA_SPARSE_SCHUR : B200BA_ITERATIVE_SCHUR);
+    if (nimg <= 0) for (int i = 0; i < NP; ++i) nimg += used[i] ? 1 : 0;
+    L.lst = nimg <= 50 ? B200BA_DENSE_SCHUR : (nimg <= 1000 ? B200BA_SPARSE_SCHUR : B200BA_ITERATIVE_SCHUR);
   }
-  sum->linear_solver_type_used = lst;
-  if (g_nobs_eff == 0 || neff == 0) { sum->termination_type = B200BA_CONVERGENCE; return 0; }
-  for (int k = 0; k < nvpt; ++k) {
-    vcount[k + 1] += vcount[k];
-  }
+  sum->linear_solver_type_used = L.lst;
+  if (cnt[0] == 0 || neff == 0) { L.nothing_to_solve = true; return 0; }
+  for (int k = 0; k < nvpt; ++k) vcount[k + 1] += vcount[k];
   std::vector<long long> vobs(vcount[nvpt]);
   {
     std::vector<long long> cur(vcount.begin(), vcount.end() - 1);
-    for (long long i = 0; i < NOBS; ++i) { const int pv = pt_var[p->obs_point_idx[i]]; if (pv >= 0) vobs[cur[pv]++] = i; }
+    for (long long i = 0; i < NOBS; ++i) { const int pv = L.pt_var[p->obs_point_idx[i]]; if (pv >= 0) vobs[cur[pv]++] = i; }
   }
   // rig sensors: a track that sees one variable frame twice (through two of its sensors) needs the cross terms between
   // those observations in the frame's SCHUR_JACOBI block, which ba_schur_pt_kernel forms
-  int pose_by_pt = 0;
-  if (NS > 0) {
-    for (int k = 0; k < nvpt && !pose_by_pt; ++k)
-      for (long long a = vcount[k]; a < vcount[k + 1] && !pose_by_pt; ++a) {
+  if (p->num_sensors > 0) {
+    for (int k = 0; k < nvpt && !L.pose_by_pt; ++k)
+      for (long long a = vcount[k]; a < vcount[k + 1] && !L.pose_by_pt; ++a) {
         const int pa = p->obs_pose_idx[vobs[a]];
-        if (pose_off[pa] < 0) continue;
-        for (long long b = a + 1; b < vcount[k + 1]; ++b) if (p->obs_pose_idx[vobs[b]] == pa) { pose_by_pt = 1; break; }
+        if (L.pose_off[pa] < 0) continue;
+        for (long long b = a + 1; b < vcount[k + 1]; ++b) if (p->obs_pose_idx[vobs[b]] == pa) { L.pose_by_pt = 1; break; }
       }
-  }
-  tick("group observations by point");
-  // pack whole tracks into blocks of BA_BLOCK slots.  The host only decides WHICH observation sits in which slot
-  // (s_obs); every per-slot / per-camera-order array is then built on the device from the caller's raw arrays.
-  std::vector<int> s_obs, s_lpt, blk_pt0, blk_npt, vpt_s0(nvpt), vpt_s1(nvpt), vpt_point(nvpt);
-  {
-    const size_t cap = (size_t)(nobs_eff + nobs_eff / 8 + 4 * BA_BLOCK);
-    s_obs.reserve(cap); s_lpt.reserve(cap);
   }
   if (NOBS >= (1LL << 31)) return ba_fail(-3, "problem too large for 32-bit observation indices");
-  auto push_slot = [&](long long obs, int lpt) { s_obs.push_back((int)obs); s_lpt.push_back(obs < 0 ? -1 : lpt); };
-  // variable points are renumbered: tracks of <= 32 observations first (packed so that none crosses a warp),
-  // then the longer ones (packed so that none crosses a block)
-  std::vector<int> s_seg;
-  s_seg.reserve((size_t)(nobs_eff + nobs_eff / 8 + 4 * BA_BLOCK));
-  int nblocks_warp = 0, nblocks_giant0 = 0, nblocks_giant1 = 0;
-  {
-    std::vector<int> order_pts; order_pts.reserve(nvpt);
-    std::vector<long long> olen(nvpt), ostart(nvpt);
-    for (int k = 0; k < nvpt; ++k) { olen[k] = vcount[k + 1] - vcount[k]; ostart[k] = vcount[k]; }
-    {  // short tracks: fill every 32-slot warp greedily with the longest track that still fits (length buckets), so that
-       // almost no slot is padding (a first-come packing wastes ~11% at an average track length of 6-7)
-      std::vector<std::vector<int>> bucket(33);
-      for (int k = nvpt - 1; k >= 0; --k) if (olen[k] <= 32) bucket[olen[k]].push_back(k);   // pop_back yields ascending k
-      size_t remaining = 0;
-      for (int l = 1; l <= 32; ++l) remaining += bucket[l].size();
-      while (remaining) {
-        int cap = 32;
-        while (cap > 0) {
-          int l = std::min(cap, 32);
-          while (l > 0 && bucket[l].empty()) --l;
-          if (l == 0) break;
-          order_pts.push_back(bucket[l].back()); bucket[l].pop_back(); --remaining;
-          cap -= l;
-        }
-      }
-    }
-    tick("  buckets");
-    const int nshort = (int)order_pts.size();
-    for (int k = 0; k < nvpt; ++k) if (olen[k] > 32 && olen[k] <= BA_BLOCK) order_pts.push_back(k);
-    const int nmid = (int)order_pts.size();
-    for (int k = 0; k < nvpt; ++k) if (olen[k] > BA_BLOCK) order_pts.push_back(k);
-    // renumber: new variable index = position in order_pts
-    std::vector<int> newidx(nvpt);
-    for (int n = 0; n < nvpt; ++n) newidx[order_pts[n]] = n;
-    for (long long i = 0; i < NPT; ++i) if (pt_var[i] >= 0) pt_var[i] = newidx[pt_var[i]];
-    for (long long i = 0; i < NPT; ++i) if (pt_var[i] >= 0) vpt_point[pt_var[i]] = (int)i;
-    tick("  renumber");
-    auto pad_to = [&](size_t mult) {
-      const size_t r = s_obs.size() % mult;
-      if (r) { const size_t add = mult - r; s_obs.insert(s_obs.end(), add, -1); s_lpt.insert(s_lpt.end(), add, -1); s_seg.insert(s_seg.end(), add, 0); }
-    };
-    auto append_track = [&](long long first, long long len, int n, int seg) {   // one track: observations vobs[first .. first + len)
-      const size_t at = s_obs.size();
-      s_obs.resize(at + (size_t)len); s_lpt.insert(s_lpt.end(), (size_t)len, n); s_seg.insert(s_seg.end(), (size_t)len, seg);
-      for (long long j = 0; j < len; ++j) s_obs[at + (size_t)j] = (int)vobs[first + j];
-    };
-    int cur_blk = -1;
-    auto note_block = [&](int k) {
-      const int b = (int)(s_obs.size() / BA_BLOCK);
-      while ((int)blk_pt0.size() <= b) { blk_pt0.push_back(k); blk_npt.push_back(0); }
-      blk_npt[b]++; cur_blk = b;
-    };
-    for (int n = 0; n < nshort; ++n) {
-      const int k = order_pts[n], len = (int)olen[k];
-      const int used = (int)(s_obs.size() % 32);
-      if (used + len > 32) pad_to(32);
-      note_block(n);
-      vpt_s0[n] = (int)s_obs.size();
-      const int head = (int)(s_obs.size() % 32), last = head + len - 1;
-      append_track(ostart[k], len, n, head | (last << 8));
-      vpt_s1[n] = (int)s_obs.size();
-    }
-    pad_to(BA_BLOCK);
-    nblocks_warp = (int)(s_obs.size() / BA_BLOCK);
-    for (int n = nshort; n < nmid; ++n) {
-      const int k = order_pts[n], len = (int)olen[k];
-      const int used = (int)(s_obs.size() % BA_BLOCK);
-      if (used + len > BA_BLOCK) pad_to(BA_BLOCK);
-      note_block(n);
-      vpt_s0[n] = (int)s_obs.size();
-      append_track(ostart[k], len, n, 0);
-      vpt_s1[n] = (int)s_obs.size();
-    }
-    pad_to(BA_BLOCK);
-    nblocks_giant0 = (int)(s_obs.size() / BA_BLOCK);
-    for (int n = nmid; n < nvpt; ++n) {   // tracks longer than a block: laid out back to back, generic kernels
-      const int k = order_pts[n];
-      vpt_s0[n] = (int)s_obs.size();
-      append_track(ostart[k], olen[k], n, 0);
-      vpt_s1[n] = (int)s_obs.size();
-    }
-    pad_to(BA_BLOCK);
-    nblocks_giant1 = (int)(s_obs.size() / BA_BLOCK);
-    (void)cur_blk;
-  }
-  tick("pack tracks into slots");
-  const int nblocks_var = nblocks_giant0;   // blocks whose tracks are eliminated in shared memory / by shuffles
-  for (long long i : const_obs) { push_slot(i, -1); s_seg.push_back(0); }
-  while (s_obs.size() % BA_BLOCK) { push_slot(-1, -1); s_seg.push_back(0); }
-  const long long nslots = (long long)s_obs.size();
-  const int nblocks = (int)(nslots / BA_BLOCK);
-  blk_pt0.resize(nblocks, nvpt); blk_npt.resize(nblocks, 0);
-  if (nslots >= (1LL << 31)) return ba_fail(-3, "problem too large for 32-bit slot indices");
-  if (nc >= (1 << (wide ? 17 : 19)) - 1) return ba_fail(-3, wide ? "camera-side dimension above 2^17 is not supported with wide camera blocks" : "camera-side dimension above 2^19 is not supported");
-  tick("slot arrays");
-  if (host_only) {
-    if (g_ba_layout_out) {
-      BaHostLayout& L = *g_ba_layout_out;
-      L.s_obs = s_obs; L.s_lpt = s_lpt; L.s_seg = s_seg; L.vpt_s0 = vpt_s0; L.vpt_s1 = vpt_s1; L.vpt_point = vpt_point;
-      L.nblocks_warp = nblocks_warp; L.nblocks_var = nblocks_var; L.nblocks_giant0 = nblocks_giant0; L.nblocks_giant1 = nblocks_giant1;
-      L.nc = nc; L.nvpt = nvpt; L.dkmax = dkmax;
-      L.num_residuals = sum->num_residuals; L.num_effective_parameters = sum->num_effective_parameters;
-    }
-    sum->setup_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_setup0).count();
-    return ba_fail(-102, "B200BA_HOST_ONLY: stopped after the host flattening");
-  }
-  // ---------------------------------------------------------------- device setup
-  BaDev D; memset(&D, 0, sizeof(D));
-  int DCsel = 6 + dkmax;
-  if (wide) DCsel = dkmax <= 8 ? 14 : (dkmax <= 12 ? 18 : (dkmax <= 16 ? 22 : 28));
-  else if (dkmax > BA_MAXDK) return ba_fail(-3, "internal: narrow layout with a camera block wider than five");
-  D.nposes = NP; D.ncams = NCAM; D.npts = (int)NPT; D.nvpt = nvpt; D.nc = nc; D.DC = DCsel; D.nblocks = nblocks;
-  D.wide = wide ? 1 : 0; D.nsensors = NS;
-  D.nblocks_var = nblocks_var; D.nslots = nslots; D.loss_type = o->loss_function_type; D.loss_scale = o->loss_function_scale;
-  D.nblk = nblk;
-  std::vector<double> h_poses(p->poses, p->poses + 7 * (size_t)NP), h_cams(p->camera_params, p->camera_params + ncamparams),
-      h_pts(p->points, p->points + 3 * (size_t)NPT);
-  // ParameterizeRigsAndFrames normalises the quaternions of parameterised frames (bundle_adjustment_ceres.cc:514)
-  for (int i = 0; i < NP; ++i) if (pose_off[i] >= 0) { double* q = h_poses.data() + 7 * (size_t)i; const double n = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]); for (int k = 0; k < 4; ++k) q[k] /= n; }
-  BA_CUDA(pool.upload(&D.poses, h_poses, st)); BA_CUDA(pool.upload(&D.cams, h_cams, st)); BA_CUDA(pool.upload(&D.pts, h_pts, st));
-  BA_CUDA(pool.alloc(&D.nposes_, h_poses.size())); BA_CUDA(pool.alloc(&D.ncams_, h_cams.size())); BA_CUDA(pool.alloc(&D.npts_, h_pts.size()));
-  { int* t; BA_CUDA(pool.upload(&t, pose_off, st)); D.pose_off = t; }
-  { unsigned char* t; BA_CUDA(pool.upload(&t, pose_mask, st)); D.pose_mask = t; }
-  { int* t; BA_CUDA(pool.upload(&t, cam_model, st)); D.cam_model = t; }
-  { int* t; BA_CUDA(pool.upload(&t, cam_poff, st)); D.cam_poff = t; }
-  { int* t; BA_CUDA(pool.upload(&t, cam_off, st)); D.cam_off = t; }
-  { int* t; BA_CUDA(pool.upload(&t, cam_nvar, st)); D.cam_nvar = t; }
-  { signed char* t; BA_CUDA(pool.upload(&t, cam_var, st)); D.cam_var = t; }
-  { int* t; BA_CUDA(pool.upload(&t, cam_width, st)); D.cam_width = t; }
-  { int* t; BA_CUDA(pool.upload(&t, cam_sensor, st)); D.cam_sensor = t; }
-  { int* t; BA_CUDA(pool.upload(&t, cam_ns, st)); D.cam_ns = t; }
-  { int* t; BA_CUDA(pool.upload(&t, sens_cam, st)); D.sens_cam = t; }
-  { int* t; BA_CUDA(pool.upload(&t, blk_split, st)); D.blk_split = t; }
-  std::vector<double> h_sens(p->sensor_from_rig ? p->sensor_from_rig : nullptr, p->sensor_from_rig ? p->sensor_from_rig + 7 * (size_t)NS : nullptr);
-  h_sens.resize(7 * (size_t)NS, 0.0);
-  for (int k = 0; k < NS; ++k) if (sens_cam[k] >= 0 && cam_ns[sens_cam[k]]) { double* q = h_sens.data() + 7 * (size_t)k; const double n = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]); for (int c = 0; c < 4; ++c) q[c] /= n; }
-  BA_CUDA(pool.upload(&D.sensors, h_sens, st)); BA_CUDA(pool.alloc(&D.nsensors_, h_sens.size()));
-  if (NS) BA_CUDA(cudaMemcpyAsync(D.nsensors_, D.sensors, sizeof(double) * h_sens.size(), cudaMemcpyDeviceToDevice, st));
-  { int* t; BA_CUDA(pool.upload(&t, pt_var, st)); D.pt_var = t; }
-  { int* t; BA_CUDA(pool.upload(&t, vpt_point, st)); D.vpt_point = t; }
-  { int* t; BA_CUDA(pool.upload(&t, s_lpt, st)); D.s_lpt = t; }
-  { int* t; BA_CUDA(pool.upload(&t, s_seg, st)); D.s_seg = t; }
-  // per-slot arrays, (camera, pose) order, runs: built on the device from the caller's arrays
-  const long long nobs_c = nobs_eff;   // every non-padding slot is an observation connected to a variable block
-  const long long nobs_c_pad = (nobs_c + BA_BLOCK - 1) / BA_BLOCK * BA_BLOCK;
+  ba_pack_tracks(vcount, vobs, const_obs, L);
+  if ((long long)L.s_obs.size() >= (1LL << 31)) return ba_fail(-3, "problem too large for 32-bit slot indices");
+  if (L.nc >= (1 << (L.wide ? 17 : 19)) - 1) return ba_fail(-3, L.wide ? "camera-side dimension above 2^17 is not supported with wide camera blocks" : "camera-side dimension above 2^19 is not supported");
+  L.DC = 6 + L.dkmax;
+  if (L.wide) L.DC = L.dkmax <= 8 ? 14 : (L.dkmax <= 12 ? 18 : (L.dkmax <= 16 ? 22 : 28));
+  else if (L.dkmax > BA_MAXDK) return ba_fail(-3, "internal: narrow layout with a camera block wider than five");
+  return 0;
+}
+// ---- device setup ----
+template <int DC> static void ba_allow_spmv_smem(const BaLayout&, cudaError_t* e) {
+  *e = cudaFuncSetAttribute(ba_schur_spmv_warp_smem_kernel<DC>, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_SPMV_SMEM_MAX);
+}
+static int ba_select_path(const b200ba_options* o, const BaLayout& L, bool sharded, int sms, BaPath& P) {
+  const int nc = L.nc;
+  const bool exact = L.lst != B200BA_ITERATIVE_SCHUR;
+  // exact reduced solves: dense Cholesky of the explicit reduced camera matrix when it is small (camera-side dimension
+  // <= BA_DENSE_MAX: the local bundle adjustments of the mapper); larger exact requests run the PCG to a 1e-12 relative
+  // residual instead
+  P.dense = exact && nc > 0 && nc <= BA_DENSE_MAX && !sharded && getenv("B200BA_NO_DENSE") == nullptr;
+  P.r_tol = exact ? 1e-12 : -1.0;
+  P.max_cg = exact ? std::max(10 * nc + 100, o->max_linear_solver_iterations) : o->max_linear_solver_iterations;
+  P.fused_pcg = nc <= BA_PCG_FUSED_MAX && getenv("B200BA_PCG_MULTI") == nullptr;
+  // r of ba_pcg_mid_kernel in (at most 160 KB of) shared memory; tests/test_ba_paths_gpu.py mirrors this threshold
+  P.mid_smem = (P.fused_pcg && (size_t)nc * sizeof(double) <= 160 * 1024 && getenv("B200BA_MID_GLOBAL") == nullptr) ? (size_t)nc * sizeof(double) : 0;
+  P.mid_staged = (P.fused_pcg && nc <= BA_PCG_T * BA_MID_EPT && getenv("B200BA_MID_PLAIN") == nullptr) ? (size_t)nc * BA_MID_STAGE_BYTES_PER_ROW : 0;
+  const char* e = getenv("B200BA_SPMV_SMEM");
+  P.spmv_smem = L.nblocks_warp && (!e || atoi(e) != 0) && sizeof(double) * (size_t)nc <= BA_SPMV_SMEM_MAX;
+  P.sms = sms;
+  // function attributes are per device: set by every solve that needs them (a process may drive several GPUs)
+  if (P.mid_smem) BA_CUDA(cudaFuncSetAttribute(ba_pcg_mid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
+  if (P.mid_staged) BA_CUDA(cudaFuncSetAttribute(ba_pcg_mid_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_PCG_T * BA_MID_EPT * BA_MID_STAGE_BYTES_PER_ROW));
+  cudaError_t spmv_attr = cudaSuccess;
+  if (P.spmv_smem && sizeof(double) * (size_t)nc > 48 * 1024) BA_DISPATCH_DC(ba_allow_spmv_smem, L, &spmv_attr);
+  BA_CUDA(spmv_attr);
+  return 0;
+}
+static void ba_normalize_quat(double* q) { const double n = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]); for (int k = 0; k < 4; ++k) q[k] /= n; }
+// The per-slot arrays and the camera order, built on the device from the caller's arrays: a stable radix sort of the
+// slots by (camera, pose), then runs of equal (camera, pose) and the chunks of the camera-block builds on the host.
+static int ba_setup_order(const BaLayout& L, const b200ba_problem* p, long long nobs_c_pad, BaPool& pool, cudaStream_t st, BaDev& D) {
+  const long long NOBS = p->num_observations, nslots = D.nslots;
+  const long long nobs_c = L.nobs_eff;   // every non-padding slot is an observation connected to a variable block
   std::vector<int4> runs, chunks, chunks_off;
   std::vector<int2> runs_pc;
-  int intr_by_pt = 0;
-  {
-    int *d_sobs, *d_opose, *d_ocam, *d_opt, *d_val, *d_c2s, *d_head, *d_incl, *d_run_start;
-    double* d_oxy;
-    unsigned long long *d_key, *d_key_sorted, *d_run_key;
-    BA_CUDA(pool.upload(&d_sobs, s_obs, st));
-    BA_CUDA(pool.alloc(&d_opose, (size_t)NOBS)); BA_CUDA(pool.alloc(&d_ocam, (size_t)NOBS)); BA_CUDA(pool.alloc(&d_opt, (size_t)NOBS)); BA_CUDA(pool.alloc(&d_oxy, 2 * (size_t)NOBS));
-    BA_CUDA(cudaMemcpyAsync(d_opose, p->obs_pose_idx, sizeof(int) * (size_t)NOBS, cudaMemcpyHostToDevice, st));
-    BA_CUDA(cudaMemcpyAsync(d_ocam, p->obs_camera_idx, sizeof(int) * (size_t)NOBS, cudaMemcpyHostToDevice, st));
-    BA_CUDA(cudaMemcpyAsync(d_opt, p->obs_point_idx, sizeof(int) * (size_t)NOBS, cudaMemcpyHostToDevice, st));
-    BA_CUDA(cudaMemcpyAsync(d_oxy, p->obs_xy, sizeof(double) * 2 * (size_t)NOBS, cudaMemcpyHostToDevice, st));
-    int *t_pose, *t_cam, *t_pt, *t_s2c, *t_crun; double *t_xy, *t_xyC; int2* t_cpack; int4* t_spack;
-    BA_CUDA(pool.alloc(&t_pose, (size_t)nslots)); BA_CUDA(pool.alloc(&t_cam, (size_t)nslots)); BA_CUDA(pool.alloc(&t_pt, (size_t)nslots));
-    BA_CUDA(pool.alloc(&t_xy, 2 * (size_t)nslots)); BA_CUDA(pool.alloc(&t_s2c, (size_t)nslots)); BA_CUDA(pool.alloc(&t_spack, (size_t)nslots));
-    BA_CUDA(pool.alloc(&t_crun, (size_t)nobs_c_pad)); BA_CUDA(pool.alloc(&t_xyC, 2 * (size_t)nobs_c_pad)); BA_CUDA(pool.alloc(&t_cpack, (size_t)nobs_c_pad));
-    BA_CUDA(pool.alloc(&d_key, (size_t)nslots)); BA_CUDA(pool.alloc(&d_key_sorted, (size_t)nslots)); BA_CUDA(pool.alloc(&d_val, (size_t)nslots)); BA_CUDA(pool.alloc(&d_c2s, (size_t)nslots));
-    BA_CUDA(pool.alloc(&d_head, (size_t)nobs_c_pad)); BA_CUDA(pool.alloc(&d_incl, (size_t)nobs_c_pad));
-    const unsigned sb = (unsigned)((nslots + 255) / 256), cb = (unsigned)((nobs_c_pad + 255) / 256);
-    ba_setup_slot_kernel<<<sb, 256, 0, st>>>(nslots, d_sobs, d_opose, d_ocam, d_opt, d_oxy, t_pose, t_cam, t_pt, t_xy, d_key, d_val);
-    // stable radix sort by (camera, pose): ties keep slot order, padding (key = ~0) ends up behind the nobs_c observations
-    int cam_bits = 1; while ((1LL << cam_bits) < NCAM) ++cam_bits;
-    size_t tmp_bytes = 0, tmp2 = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, d_key, d_key_sorted, d_val, d_c2s, (int)nslots, 0, 64, st);
-    cub::DeviceScan::InclusiveSum(nullptr, tmp2, d_head, d_incl, (int)nobs_c_pad, st);
-    tmp_bytes = std::max(tmp_bytes, tmp2);
-    unsigned char* d_tmp; BA_CUDA(pool.alloc(&d_tmp, tmp_bytes));
-    BA_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, d_key, d_key_sorted, d_val, d_c2s, (int)nslots, 0, 64, st));
-    (void)cam_bits;
-    BA_CUDA(cudaMemsetAsync(t_s2c, 0xff, sizeof(int) * (size_t)nslots, st));
-    BA_CUDA(cudaMemsetAsync(d_head, 0, sizeof(int) * (size_t)nobs_c_pad, st));
-    BA_CUDA(cudaMemsetAsync(t_crun, 0xff, sizeof(int) * (size_t)nobs_c_pad, st));
-    if (nobs_c_pad) ba_setup_cam_kernel<<<cb, 256, 0, st>>>(nobs_c, nobs_c_pad, nslots, d_key_sorted, d_c2s, t_pt, D.s_lpt, t_xy, t_s2c, t_cpack, t_xyC, d_head);
-    if (nobs_c) BA_CUDA(cub::DeviceScan::InclusiveSum(d_tmp, tmp_bytes, d_head, d_incl, (int)nobs_c, st));
-    int nruns = 0;
-    if (nobs_c) {
-      BA_CUDA(cudaMemcpyAsync(&nruns, d_incl + (nobs_c - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
-      BA_CUDA(cudaStreamSynchronize(st));
-    }
-    BA_CUDA(pool.alloc(&d_run_start, (size_t)nruns + 1)); BA_CUDA(pool.alloc(&d_run_key, (size_t)nruns + 1));
-    if (nobs_c) ba_setup_run_kernel<<<cb, 256, 0, st>>>(nobs_c, d_incl, t_crun, d_head, d_key_sorted, d_run_start, d_run_key);
-    ba_setup_pack_kernel<<<sb, 256, 0, st>>>(nslots, t_pose, t_cam, D.s_lpt, D.s_seg, t_s2c, D.pose_off, D.cam_off, D.cam_width, D.wide, t_spack);
-    std::vector<int> run_start((size_t)nruns + 1);
-    std::vector<unsigned long long> run_key((size_t)nruns + 1);
-    if (nruns) {
-      BA_CUDA(cudaMemcpyAsync(run_start.data(), d_run_start, sizeof(int) * (size_t)nruns, cudaMemcpyDeviceToHost, st));
-      BA_CUDA(cudaMemcpyAsync(run_key.data(), d_run_key, sizeof(unsigned long long) * (size_t)nruns, cudaMemcpyDeviceToHost, st));
-      BA_CUDA(cudaStreamSynchronize(st));
-    }
-    run_start[nruns] = (int)nobs_c;
-    // runs of equal (camera, pose); chunks (<= BA_CHUNK observations of one pose block / one intrinsics block)
-    // chunk word: first column | width << 8 | first row inside the block << 16 | block width << 24
-    auto add_chunks = [&](long long k0, long long k1, int out, int comp0, int ncomp, int lr0, int bw) {
-      for (long long c0 = k0; c0 < k1; c0 += BA_CHUNK) chunks.push_back(make_int4((int)c0, (int)std::min<long long>(c0 + BA_CHUNK, k1), out, comp0 | (ncomp << 8) | (lr0 << 16) | (bw << 24)));
-    };
-    auto add_pair_chunks = [&](long long k0, long long k1, int blk_off, int cA, int nA, int cB, int nB) {
-      for (long long c0 = k0; c0 < k1; c0 += BA_CHUNK) chunks_off.push_back(make_int4((int)c0, (int)std::min<long long>(c0 + BA_CHUNK, k1), blk_off, cA | (nA << 8) | (cB << 16) | (nB << 24)));
-    };
-    long long cam_start = 0;
-    for (int r = 0; r < nruns; ++r) {
-      const int pose = (int)(run_key[r] & 0xffffffffu), cam = (int)(run_key[r] >> 32);
-      const long long k = run_start[r], e = run_start[r + 1];
-      runs.push_back(make_int4(pose_off[pose], cam_off[cam], cam_width[cam], 0));
-      runs_pc.push_back(make_int2(pose, cam));
-      if (pose_off[pose] >= 0) add_chunks(k, e, pose_off[pose], 0, 6, 0, 6);
-      const bool cam_ends = (r + 1 == nruns) || (int)(run_key[r + 1] >> 32) != cam;
-      // a variable camera block seen from several poses: some track may see it twice -> the camera blocks of
-      // the preconditioner need the cross terms between observations of one point (ba_schur_pt_kernel)
-      if (!cam_ends && cam_off[cam] >= 0) intr_by_pt = 1;
-      if (cam_ends) {
-        if (cam_off[cam] >= 0) {
-          const int w = cam_width[cam];
-          for (int a = 0; a < w; a += 6) {   // 6-column ranges of the block: diagonal ranges here, pairs of ranges separately
-            add_chunks(cam_start, e, cam_off[cam] + a, 6 + a, std::min(6, w - a), a, w);
-            for (int b = a + 6; b < w; b += 6) add_pair_chunks(cam_start, e, cam_off[cam], 6 + a, std::min(6, w - a), 6 + b, std::min(6, w - b));
-          }
+  int *d_sobs, *d_opose, *d_ocam, *d_opt, *d_val, *d_c2s, *d_head, *d_incl, *d_run_start;
+  double* d_oxy;
+  unsigned long long *d_key, *d_key_sorted, *d_run_key;
+  BA_CUDA(pool.upload(&d_sobs, L.s_obs, st));
+  BA_CUDA(pool.alloc(&d_opose, (size_t)NOBS)); BA_CUDA(pool.alloc(&d_ocam, (size_t)NOBS)); BA_CUDA(pool.alloc(&d_opt, (size_t)NOBS)); BA_CUDA(pool.alloc(&d_oxy, 2 * (size_t)NOBS));
+  BA_CUDA(cudaMemcpyAsync(d_opose, p->obs_pose_idx, sizeof(int) * (size_t)NOBS, cudaMemcpyHostToDevice, st));
+  BA_CUDA(cudaMemcpyAsync(d_ocam, p->obs_camera_idx, sizeof(int) * (size_t)NOBS, cudaMemcpyHostToDevice, st));
+  BA_CUDA(cudaMemcpyAsync(d_opt, p->obs_point_idx, sizeof(int) * (size_t)NOBS, cudaMemcpyHostToDevice, st));
+  BA_CUDA(cudaMemcpyAsync(d_oxy, p->obs_xy, sizeof(double) * 2 * (size_t)NOBS, cudaMemcpyHostToDevice, st));
+  int *t_pose, *t_cam, *t_pt, *t_s2c, *t_crun; double *t_xy, *t_xyC; int2* t_cpack; int4* t_spack;
+  BA_CUDA(pool.alloc(&t_pose, (size_t)nslots)); BA_CUDA(pool.alloc(&t_cam, (size_t)nslots)); BA_CUDA(pool.alloc(&t_pt, (size_t)nslots));
+  BA_CUDA(pool.alloc(&t_xy, 2 * (size_t)nslots)); BA_CUDA(pool.alloc(&t_s2c, (size_t)nslots)); BA_CUDA(pool.alloc(&t_spack, (size_t)nslots));
+  BA_CUDA(pool.alloc(&t_crun, (size_t)nobs_c_pad)); BA_CUDA(pool.alloc(&t_xyC, 2 * (size_t)nobs_c_pad)); BA_CUDA(pool.alloc(&t_cpack, (size_t)nobs_c_pad));
+  BA_CUDA(pool.alloc(&d_key, (size_t)nslots)); BA_CUDA(pool.alloc(&d_key_sorted, (size_t)nslots)); BA_CUDA(pool.alloc(&d_val, (size_t)nslots)); BA_CUDA(pool.alloc(&d_c2s, (size_t)nslots));
+  BA_CUDA(pool.alloc(&d_head, (size_t)nobs_c_pad)); BA_CUDA(pool.alloc(&d_incl, (size_t)nobs_c_pad));
+  const unsigned sb = (unsigned)((nslots + 255) / 256), cb = (unsigned)((nobs_c_pad + 255) / 256);
+  ba_setup_slot_kernel<<<sb, 256, 0, st>>>(nslots, d_sobs, d_opose, d_ocam, d_opt, d_oxy, t_pose, t_cam, t_pt, t_xy, d_key, d_val);
+  // stable radix sort by (camera, pose): ties keep slot order, padding (key = ~0) ends up behind the nobs_c observations
+  size_t tmp_bytes = 0, tmp2 = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, d_key, d_key_sorted, d_val, d_c2s, (int)nslots, 0, 64, st);
+  cub::DeviceScan::InclusiveSum(nullptr, tmp2, d_head, d_incl, (int)nobs_c_pad, st);
+  tmp_bytes = std::max(tmp_bytes, tmp2);
+  unsigned char* d_tmp; BA_CUDA(pool.alloc(&d_tmp, tmp_bytes));
+  BA_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, d_key, d_key_sorted, d_val, d_c2s, (int)nslots, 0, 64, st));
+  BA_CUDA(cudaMemsetAsync(t_s2c, 0xff, sizeof(int) * (size_t)nslots, st));
+  BA_CUDA(cudaMemsetAsync(d_head, 0, sizeof(int) * (size_t)nobs_c_pad, st));
+  BA_CUDA(cudaMemsetAsync(t_crun, 0xff, sizeof(int) * (size_t)nobs_c_pad, st));
+  if (nobs_c_pad) ba_setup_cam_kernel<<<cb, 256, 0, st>>>(nobs_c, nobs_c_pad, nslots, d_key_sorted, d_c2s, t_pt, D.s_lpt, t_xy, t_s2c, t_cpack, t_xyC, d_head);
+  if (nobs_c) BA_CUDA(cub::DeviceScan::InclusiveSum(d_tmp, tmp_bytes, d_head, d_incl, (int)nobs_c, st));
+  int nruns = 0;
+  if (nobs_c) {
+    BA_CUDA(cudaMemcpyAsync(&nruns, d_incl + (nobs_c - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
+    BA_CUDA(cudaStreamSynchronize(st));
+  }
+  BA_CUDA(pool.alloc(&d_run_start, (size_t)nruns + 1)); BA_CUDA(pool.alloc(&d_run_key, (size_t)nruns + 1));
+  if (nobs_c) ba_setup_run_kernel<<<cb, 256, 0, st>>>(nobs_c, d_incl, t_crun, d_head, d_key_sorted, d_run_start, d_run_key);
+  ba_setup_pack_kernel<<<sb, 256, 0, st>>>(nslots, t_pose, t_cam, D.s_lpt, D.s_seg, t_s2c, D.pose_off, D.cam_off, D.cam_width, D.wide, t_spack);
+  std::vector<int> run_start((size_t)nruns + 1);
+  std::vector<unsigned long long> run_key((size_t)nruns + 1);
+  if (nruns) {
+    BA_CUDA(cudaMemcpyAsync(run_start.data(), d_run_start, sizeof(int) * (size_t)nruns, cudaMemcpyDeviceToHost, st));
+    BA_CUDA(cudaMemcpyAsync(run_key.data(), d_run_key, sizeof(unsigned long long) * (size_t)nruns, cudaMemcpyDeviceToHost, st));
+    BA_CUDA(cudaStreamSynchronize(st));
+  }
+  run_start[nruns] = (int)nobs_c;
+  // runs of equal (camera, pose); chunks (<= BA_CHUNK observations of one pose block / one intrinsics block)
+  // chunk word: first column | width << 8 | first row inside the block << 16 | block width << 24
+  auto add_chunks = [&](long long k0, long long k1, int out, int comp0, int ncomp, int lr0, int bw) {
+    for (long long c0 = k0; c0 < k1; c0 += BA_CHUNK) chunks.push_back(make_int4((int)c0, (int)std::min<long long>(c0 + BA_CHUNK, k1), out, comp0 | (ncomp << 8) | (lr0 << 16) | (bw << 24)));
+  };
+  auto add_pair_chunks = [&](long long k0, long long k1, int blk_off, int cA, int nA, int cB, int nB) {
+    for (long long c0 = k0; c0 < k1; c0 += BA_CHUNK) chunks_off.push_back(make_int4((int)c0, (int)std::min<long long>(c0 + BA_CHUNK, k1), blk_off, cA | (nA << 8) | (cB << 16) | (nB << 24)));
+  };
+  long long cam_start = 0;
+  for (int r = 0; r < nruns; ++r) {
+    const int pose = (int)(run_key[r] & 0xffffffffu), cam = (int)(run_key[r] >> 32);
+    const long long k = run_start[r], e = run_start[r + 1];
+    runs.push_back(make_int4(L.pose_off[pose], L.cam_off[cam], L.cam_width[cam], 0));
+    runs_pc.push_back(make_int2(pose, cam));
+    if (L.pose_off[pose] >= 0) add_chunks(k, e, L.pose_off[pose], 0, 6, 0, 6);
+    const bool cam_ends = (r + 1 == nruns) || (int)(run_key[r + 1] >> 32) != cam;
+    // a variable camera block seen from several poses: some track may see it twice -> the camera blocks of
+    // the preconditioner need the cross terms between observations of one point (ba_schur_pt_kernel)
+    if (!cam_ends && L.cam_off[cam] >= 0) D.intr_by_pt = 1;
+    if (cam_ends) {
+      if (L.cam_off[cam] >= 0) {
+        const int w = L.cam_width[cam];
+        for (int a = 0; a < w; a += 6) {   // 6-column ranges of the block: diagonal ranges here, pairs of ranges separately
+          add_chunks(cam_start, e, L.cam_off[cam] + a, 6 + a, std::min(6, w - a), a, w);
+          for (int b = a + 6; b < w; b += 6) add_pair_chunks(cam_start, e, L.cam_off[cam], 6 + a, std::min(6, w - a), 6 + b, std::min(6, w - b));
         }
-        cam_start = e;
       }
+      cam_start = e;
     }
-    D.s_pose = t_pose; D.s_cam = t_cam; D.s_pt = t_pt; D.s_xy = t_xy; D.s2c = t_s2c; D.s_pack = t_spack;
-    D.c_run = t_crun; D.xyC = t_xyC; D.c_pack = t_cpack;
   }
-  { int* t; BA_CUDA(pool.upload(&t, blk_pt0, st)); D.blk_pt0 = t; }
-  { int* t; BA_CUDA(pool.upload(&t, blk_npt, st)); D.blk_npt = t; }
-  { int* t; BA_CUDA(pool.upload(&t, vpt_s0, st)); D.vpt_s0 = t; }
-  { int* t; BA_CUDA(pool.upload(&t, vpt_s1, st)); D.vpt_s1 = t; }
-  { int* t; BA_CUDA(pool.upload(&t, blk_start, st)); D.blk_start = t; }
-  { int* t; BA_CUDA(pool.upload(&t, blk_pack, st)); D.blk_pack = t; }
-  { int* t; BA_CUDA(pool.upload(&t, off2blk, st)); D.off2blk = t; }
-  {
-    std::vector<int4> row_info((size_t)nc);
-    for (int i = 0; i < nc; ++i) {
-      const int b = off2blk[i], n = blk_start[b + 1] - blk_start[b], l = i - blk_start[b];
-      row_info[i] = make_int4(blk_start[b], blk_pack[b] + l * n, n, 0);
-    }
-    int4* t; BA_CUDA(pool.upload(&t, row_info, st)); D.row_info = t;
+  D.s_pose = t_pose; D.s_cam = t_cam; D.s_pt = t_pt; D.s_xy = t_xy; D.s2c = t_s2c; D.s_pack = t_spack;
+  D.c_run = t_crun; D.xyC = t_xyC; D.c_pack = t_cpack;
+  BA_CUDA(pool.upload(&D.runs_pc, runs_pc, st));
+  BA_CUDA(pool.upload(&D.chunks, chunks, st));
+  BA_CUDA(pool.upload(&D.chunks_off, chunks_off, st));
+  BA_CUDA(pool.upload(&D.runs, runs, st));
+  D.nchunks = (int)chunks.size(); D.nchunks_off = (int)chunks_off.size(); D.nobs_c = nobs_c;
+  return 0;
+}
+// Everything the device holds for one solve: the parameters (current and candidate), the maps of the layout, the slot
+// and camera-order arrays and the scratch of the LM and PCG loops.  comm: set for a sharded solve.
+static int ba_upload(const BaLayout& L, const b200ba_options* o, const b200ba_problem* p, const BaPath& path,
+                     b200ba_comm* comm, BaPool& pool, cudaStream_t st, BaDev& D) {
+  const int NP = p->num_poses, NS = p->num_sensors, nc = L.nc, nvpt = L.nvpt, pack = L.pack;
+  const long long NPT = p->num_points, nslots = (long long)L.s_obs.size();
+  memset(&D, 0, sizeof(D));
+  D.nposes = NP; D.ncams = p->num_cameras; D.npts = (int)NPT; D.nvpt = nvpt; D.nc = nc; D.DC = L.DC; D.nblocks = L.nblocks;
+  D.wide = L.wide ? 1 : 0; D.nsensors = NS;
+  D.nblocks_var = L.nblocks_giant0;   // blocks whose tracks are eliminated in shared memory / by shuffles
+  D.nslots = nslots; D.loss_type = o->loss_function_type; D.loss_scale = o->loss_function_scale;
+  D.nblk = L.nblk;
+  std::vector<double> h_poses(p->poses, p->poses + 7 * (size_t)NP), h_cams(p->camera_params, p->camera_params + L.ncamparams),
+      h_pts(p->points, p->points + 3 * (size_t)NPT), h_sens(p->sensor_from_rig, p->sensor_from_rig + 7 * (size_t)NS);
+  // ParameterizeRigsAndFrames normalises the quaternions of parameterised frames and sensors (bundle_adjustment_ceres.cc:514)
+  for (int i = 0; i < NP; ++i) if (L.pose_off[i] >= 0) ba_normalize_quat(h_poses.data() + 7 * (size_t)i);
+  for (int k = 0; k < NS; ++k) if (L.sens_cam[k] >= 0 && L.cam_ns[L.sens_cam[k]]) ba_normalize_quat(h_sens.data() + 7 * (size_t)k);
+  BA_CUDA(pool.upload(&D.poses, h_poses, st)); BA_CUDA(pool.upload(&D.cams, h_cams, st)); BA_CUDA(pool.upload(&D.pts, h_pts, st));
+  BA_CUDA(pool.alloc(&D.nposes_, h_poses.size())); BA_CUDA(pool.alloc(&D.ncams_, h_cams.size())); BA_CUDA(pool.alloc(&D.npts_, h_pts.size()));
+  BA_CUDA(pool.upload(&D.pose_off, L.pose_off, st));
+  BA_CUDA(pool.upload(&D.pose_mask, L.pose_mask, st));
+  BA_CUDA(pool.upload(&D.cam_model, L.cam_model, st));
+  BA_CUDA(pool.upload(&D.cam_poff, L.cam_poff, st));
+  BA_CUDA(pool.upload(&D.cam_off, L.cam_off, st));
+  BA_CUDA(pool.upload(&D.cam_nvar, L.cam_nvar, st));
+  BA_CUDA(pool.upload(&D.cam_var, L.cam_var, st));
+  BA_CUDA(pool.upload(&D.cam_width, L.cam_width, st));
+  BA_CUDA(pool.upload(&D.cam_sensor, L.cam_sensor, st));
+  BA_CUDA(pool.upload(&D.cam_ns, L.cam_ns, st));
+  BA_CUDA(pool.upload(&D.sens_cam, L.sens_cam, st));
+  BA_CUDA(pool.upload(&D.blk_split, L.blk_split, st));
+  BA_CUDA(pool.upload(&D.sensors, h_sens, st)); BA_CUDA(pool.alloc(&D.nsensors_, h_sens.size()));
+  if (NS) BA_CUDA(cudaMemcpyAsync(D.nsensors_, D.sensors, sizeof(double) * h_sens.size(), cudaMemcpyDeviceToDevice, st));
+  BA_CUDA(pool.upload(&D.pt_var, L.pt_var, st));
+  BA_CUDA(pool.upload(&D.vpt_point, L.vpt_point, st));
+  BA_CUDA(pool.upload(&D.s_lpt, L.s_lpt, st));
+  BA_CUDA(pool.upload(&D.s_seg, L.s_seg, st));
+  const long long nobs_c_pad = (L.nobs_eff + BA_BLOCK - 1) / BA_BLOCK * BA_BLOCK;
+  BA_TRY(ba_setup_order(L, p, nobs_c_pad, pool, st, D));
+  BA_CUDA(pool.upload(&D.blk_pt0, L.blk_pt0, st));
+  BA_CUDA(pool.upload(&D.blk_npt, L.blk_npt, st));
+  BA_CUDA(pool.upload(&D.vpt_s0, L.vpt_s0, st));
+  BA_CUDA(pool.upload(&D.vpt_s1, L.vpt_s1, st));
+  BA_CUDA(pool.upload(&D.blk_start, L.blk_start, st));
+  BA_CUDA(pool.upload(&D.blk_pack, L.blk_pack, st));
+  BA_CUDA(pool.upload(&D.off2blk, L.off2blk, st));
+  std::vector<int4> row_info((size_t)nc);
+  for (int i = 0; i < nc; ++i) {
+    const int b = L.off2blk[i], n = L.blk_start[b + 1] - L.blk_start[b], l = i - L.blk_start[b];
+    row_info[i] = make_int4(L.blk_start[b], L.blk_pack[b] + l * n, n, 0);
   }
+  BA_CUDA(pool.upload(&D.row_info, row_info, st));
   BA_CUDA(pool.alloc(&D.Jc, (size_t)2 * D.DC * nslots)); BA_CUDA(pool.alloc(&D.Jp, (size_t)6 * nslots));
   BA_CUDA(pool.alloc(&D.JcC, (size_t)2 * D.DC * nobs_c_pad)); BA_CUDA(pool.alloc(&D.u, (size_t)nobs_c_pad)); BA_CUDA(pool.alloc(&D.rC, (size_t)2 * nobs_c_pad)); BA_CUDA(pool.alloc(&D.JpC, (size_t)6 * nobs_c_pad));
-  { int2* t; BA_CUDA(pool.upload(&t, runs_pc, st)); D.runs_pc = t; }
-  D.intr_by_pt = intr_by_pt;
-  D.pose_by_pt = pose_by_pt;
-  D.nblocks_warp = nblocks_warp; D.nblocks_giant0 = nblocks_giant0; D.nblocks_giant1 = nblocks_giant1;
+  D.pose_by_pt = L.pose_by_pt;
+  D.nblocks_warp = L.nblocks_warp; D.nblocks_giant0 = L.nblocks_giant0; D.nblocks_giant1 = L.nblocks_giant1;
   BA_CUDA(pool.alloc(&D.zg, (size_t)3 * nvpt));
-  { int4* t; BA_CUDA(pool.upload(&t, chunks, st)); D.chunks = t; }
-  { int4* t; BA_CUDA(pool.upload(&t, chunks_off, st)); D.chunks_off = t; D.nchunks_off = (int)chunks_off.size(); }
-  { int4* t; BA_CUDA(pool.upload(&t, runs, st)); D.runs = t; }
-  D.nchunks = (int)chunks.size(); D.nobs_c = nobs_c; BA_CUDA(pool.alloc(&D.r, (size_t)2 * nslots)); BA_CUDA(pool.alloc(&D.cost_slot, (size_t)nslots));
+  BA_CUDA(pool.alloc(&D.r, (size_t)2 * nslots)); BA_CUDA(pool.alloc(&D.cost_slot, (size_t)nslots));
   BA_CUDA(pool.alloc(&D.scale_c, (size_t)nc)); BA_CUDA(pool.alloc(&D.scale_p, (size_t)3 * nvpt));
   BA_CUDA(pool.alloc(&D.Hpp, (size_t)6 * nvpt)); BA_CUDA(pool.alloc(&D.Hpp_inv, (size_t)6 * nvpt)); BA_CUDA(pool.alloc(&D.gp, (size_t)3 * nvpt));
   BA_CUDA(pool.alloc(&D.diag_p, (size_t)3 * nvpt)); BA_CUDA(pool.alloc(&D.Dp2, (size_t)3 * nvpt)); BA_CUDA(pool.alloc(&D.dp, (size_t)3 * nvpt));
   BA_CUDA(pool.alloc(&D.gc, (size_t)nc)); BA_CUDA(pool.alloc(&D.diag_c, (size_t)nc)); BA_CUDA(pool.alloc(&D.Dc2, (size_t)nc)); BA_CUDA(pool.alloc(&D.rhs, (size_t)nc));
-  if (sharded) {   // symmetric peer buffers for the latency-bound collectives of the LM / PCG loops (kept by the communicator)
+  if (comm) {   // symmetric peer buffers for the latency-bound collectives of the LM / PCG loops (kept by the communicator)
     const size_t grouped = (size_t)nc + (size_t)pack + 1;
     ba_p2p_ensure(comm, grouped * sizeof(double) <= BA_P2P_MAX_BYTES ? grouped : ((size_t)nc * sizeof(double) <= BA_P2P_MAX_BYTES ? (size_t)nc : 4), st);
     if (getenv("B200BA_VERBOSE") && comm->rank == 0) fprintf(stderr, "[b200ba] peer-memory all-reduce: %s (cap %zu doubles)\n", comm->p2p.ok ? "on" : "off (NCCL)", comm->p2p.cap);
   }
   BA_CUDA(pool.alloc(&D.Hbb, (size_t)pack)); BA_CUDA(pool.alloc(&D.Mbb, (size_t)pack)); BA_CUDA(pool.alloc(&D.Minv, (size_t)pack));
   BA_CUDA(pool.alloc(&D.x, (size_t)nc)); BA_CUDA(pool.alloc(&D.rr, (size_t)nc)); BA_CUDA(pool.alloc(&D.z, (size_t)nc)); BA_CUDA(pool.alloc(&D.p, (size_t)nc)); BA_CUDA(pool.alloc(&D.q, (size_t)nc));
-  const bool want_exact = (lst != B200BA_ITERATIVE_SCHUR);
-  // exact reduced solves: dense Cholesky of the explicit reduced camera matrix when it is small (camera-side dimension
-  // <= BA_DENSE_MAX: the local bundle adjustments of the mapper); larger exact requests run the PCG to a 1e-12 relative
-  // residual instead
-  const bool dense = want_exact && nc > 0 && nc <= BA_DENSE_MAX && !sharded && getenv("B200BA_NO_DENSE") == nullptr;
-  if (dense) BA_CUDA(pool.alloc(&D.Sd, (size_t)nc * nc));
+  if (path.dense) BA_CUDA(pool.alloc(&D.Sd, (size_t)nc * nc));
   BA_CUDA(pool.alloc(&D.ctl, 1));
-  int* d_fail = &D.ctl->fail;   // part of the control block: travels with the per-iteration read
   BA_CUDA(cudaMemsetAsync(D.ctl, 0, sizeof(BaCtl), st));
   BA_CUDA(cudaMemsetAsync(D.x, 0, sizeof(double) * (nc ? nc : 1), st));
   BA_CUDA(cudaMemsetAsync(D.dp, 0, sizeof(double) * (nvpt ? 3 * (size_t)nvpt : 1), st));
   BA_CUDA(cudaStreamSynchronize(st));
-  sum->setup_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_setup0).count();
-
-  for (int i = 0; i < 4; ++i) BA_CUDA(cudaEventCreate(&guard.ev[i]));
-  const cudaEvent_t ev0 = guard.ev[0], ev1 = guard.ev[1], evs0 = guard.ev[2], evs1 = guard.ev[3];
+  return 0;
+}
+// ---- the LM loop ----
+// B200BA_PROFILE=1: device-timeline breakdown of the solve by phase (events between the launches; the interval that
+// ends at a "host" mark is GPU idle time spent waiting for the host round trip).  Diagnostic only.
+enum { PF_LIN, PF_BUILD, PF_AR_BUILD, PF_DIAG, PF_DAMP_SCHUR, PF_AR_SCHUR, PF_INVERT, PF_PCG_INIT, PF_SPMV, PF_AR_Q, PF_MID,
+       PF_HOST, PF_BACKSUB, PF_UPDATE_COST, PF_AR_COST, PF_N };
+// The phases of one solve on the device and the state they share.  Each returns 0 or a b200ba error code.  The stream
+// and events are destroyed on every return path (declared after the pool, so before its release).
+struct BaSolve {
+  const b200ba_options* o = nullptr;
+  cudaStream_t st = nullptr;
+  cudaEvent_t ev[4] = {};   // solve start and end; around the first SpMV of every PCG batch
+  BaReducer red;
+  BaPath path;
+  BaDev D;
+  int pack = 0, dkmax = 0;   // packed size of the camera-side blocks, widest camera block
+  const bool check = getenv("B200BA_CHECK") != nullptr;   // synchronise and test for asynchronous errors after every group of launches
+  const bool profile = getenv("B200BA_PROFILE") != nullptr;
+  std::vector<cudaEvent_t> pf_ev;
+  std::vector<int> pf_tag;   // phase of the interval that ends at pf_ev[k]
   int launches = 0, spmv_launches = 0;
   double spmv_ms = 0.0;
-  const int gc_blocks = (nc + 255) / 256, gp_blocks = (nvpt + 255) / 256;
+  BaCtl* h = nullptr;                           // host copy of the control block (pinned when possible)
+  BaCtl h_pageable;
+  ~BaSolve() {
+    for (cudaEvent_t e : pf_ev) cudaEventDestroy(e);
+    for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+    if (st) { cudaStreamSynchronize(st); cudaStreamDestroy(st); }
+  }
+  void mark(int tag) { if (!profile) return; cudaEvent_t e; if (cudaEventCreate(&e) != cudaSuccess) return; cudaEventRecord(e, st); pf_ev.push_back(e); pf_tag.push_back(tag); }
+  void report(int world, int lm, float solve_ms) const {
+    static const char* const names[PF_N] = {"linearize", "build (cam blocks, gradient)", "all-reduce gc+Hbb", "diag/build_pt/gradmax(+AR)",
+        "damp + schur_cam", "all-reduce rhs+Mbb", "invert blocks", "pcg init", "spmv (both passes)", "all-reduce q", "pcg mid",
+        "host round trip (GPU idle)", "backsub", "update + cost", "all-reduce cost"};
+    double acc[PF_N] = {0}; int cnt[PF_N] = {0};
+    for (size_t k = 1; k < pf_ev.size(); ++k) { float ms = 0; if (cudaEventElapsedTime(&ms, pf_ev[k - 1], pf_ev[k]) == cudaSuccess) { acc[pf_tag[k]] += ms; cnt[pf_tag[k]]++; } }
+    fprintf(stderr, "[b200ba profile] world %d, %d LM iterations, %.1f ms on the device\n", world, lm, solve_ms);
+    for (int t = 0; t < PF_N; ++t) if (cnt[t]) fprintf(stderr, "[b200ba profile] %-30s %8.2f ms %5.1f %%  n=%6d  %7.1f us each  %7.1f us / LM it\n", names[t], acc[t], 100.0 * acc[t] / solve_ms, cnt[t], 1e3 * acc[t] / cnt[t], 1e3 * acc[t] / std::max(lm, 1));
+  }
+  unsigned gc_blocks() const { return (unsigned)((D.nc + 255) / 256); }
+  unsigned gp_blocks() const { return (unsigned)((D.nvpt + 255) / 256); }
+  bool replica() const { return red.comm && red.comm->rank != 0; }   // sharded, not rank 0: replicated terms come from rank 0
+  cudaError_t zero(void* field, size_t bytes = sizeof(double)) { return cudaMemsetAsync(field, 0, bytes, st); }
+  cudaError_t read_ctl() { cudaError_t e = cudaMemcpyAsync(h, D.ctl, sizeof(BaCtl), cudaMemcpyDeviceToHost, st); if (e != cudaSuccess) return e; return cudaStreamSynchronize(st); }
+  int checkpoint(const char* label) {
+    if (!check) return 0;
+    cudaError_t e = cudaStreamSynchronize(st);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : ba_fail(-100, std::string("checkpoint ") + label + ": " + cudaGetErrorString(e));
+  }
+  int linearize(int apply_scale) {
+    BA_CUDA(zero(&D.ctl->cost));
+    BA_DISPATCH_DC(ba_launch_linearize, D, apply_scale, st);
+    mark(PF_LIN);
+    BA_CUDA(red(&D.ctl->cost, 1, ncclDouble, ncclSum));
+    mark(PF_AR_COST);
+    launches += 2;
+    return 0;
+  }
+  // iteration 0: Jacobian and jacobi scaling, then the scaled Jacobian (fp32) in both orders
+  int linearize_scaled() {
+    BA_TRY(linearize(0));
+    BA_TRY(checkpoint("linearize(0)"));
+    BA_CUDA(zero(D.scale_c, sizeof(double) * (D.nc ? D.nc : 1)));
+    BA_CUDA(zero(D.scale_p, sizeof(double) * (D.nvpt ? 3 * (size_t)D.nvpt : 1)));
+    ba_colnorm_kernel<<<D.nblocks, BA_BLOCK, 0, st>>>(D);
+    BA_CUDA(red(D.scale_c, D.nc, ncclDouble, ncclSum));
+    if (D.nc) ba_make_scale_kernel<<<gc_blocks(), 256, 0, st>>>(D.scale_c, D.nc, o->jacobi_scaling);
+    if (D.nvpt) ba_make_scale_kernel<<<(3 * D.nvpt + 255) / 256, 256, 0, st>>>(D.scale_p, 3LL * D.nvpt, o->jacobi_scaling);
+    launches += 3;
+    BA_TRY(checkpoint("colnorm"));
+    BA_TRY(linearize(1));
+    return checkpoint("linearize(1)");
+  }
+  // normal equations from the current (scaled) Jacobian: camera blocks and gradient, point blocks, gradient max-norm
+  int build() {
+    BA_CUDA(zero(D.gc, sizeof(double) * (D.nc ? D.nc : 1)));
+    BA_CUDA(zero(D.Hbb, sizeof(double) * (pack ? pack : 1)));
+    BA_CUDA(zero(&D.ctl->gmax));
+    if (D.nchunks) ba_build_cam_sorted_kernel<<<(D.nchunks + BA_SC_BLOCK / 32 - 1) / (BA_SC_BLOCK / 32), BA_SC_BLOCK, 0, st>>>(D);
+    BA_TRY(checkpoint("build_cam_sorted"));
+    if (D.nchunks_off) ba_cam_offdiag_kernel<false><<<(D.nchunks_off + BA_SC_BLOCK / 32 - 1) / (BA_SC_BLOCK / 32), BA_SC_BLOCK, 0, st>>>(D);
+    BA_TRY(checkpoint("cam_offdiag<false>"));
+    mark(PF_BUILD);
+    red.begin();
+    BA_CUDA(red(D.gc, D.nc, ncclDouble, ncclSum));
+    BA_CUDA(red(D.Hbb, pack, ncclDouble, ncclSum));
+    BA_CUDA(red.end());
+    mark(PF_AR_BUILD);
+    if (D.nc) ba_diag_from_blocks_kernel<<<gc_blocks(), 256, 0, st>>>(D);
+    if (D.nvpt) ba_build_pt_kernel<<<gp_blocks(), 256, 0, st>>>(D);
+    BA_TRY(checkpoint("diag + build_pt"));
+    { const long long n = (((long long)D.nposes + 31) & ~31LL) + (((long long)D.ncams + 31) & ~31LL) + 3LL * D.nvpt; ba_gradmax_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(D); }
+    BA_TRY(checkpoint("gradmax"));
+    launches += 4;
+    BA_CUDA(red(&D.ctl->gmax, 1, ncclDouble, ncclMax));
+    mark(PF_DIAG);
+    return 0;
+  }
+  // LM damping, the reduced camera system (rhs and camera blocks) and the inverses of its diagonal blocks
+  int damp(double radius) {
+    int* d_fail = &D.ctl->fail;   // part of the control block: travels with the per-iteration read
+    BA_CUDA(zero(d_fail, sizeof(int)));
+    if (D.nvpt) ba_damp_pt_kernel<<<gp_blocks(), 256, 0, st>>>(D, 1.0 / radius, o->min_lm_diagonal, o->max_lm_diagonal, d_fail);
+    if (D.nc) ba_damp_cam_kernel<<<gc_blocks(), 256, 0, st>>>(D, 1.0 / radius, o->min_lm_diagonal, o->max_lm_diagonal);
+    if (replica()) {  // the replicated terms (-g_c, H_bb + D) are contributed by rank 0 only
+      BA_CUDA(zero(D.rhs, sizeof(double) * (D.nc ? D.nc : 1)));
+      BA_CUDA(zero(D.Mbb, sizeof(double) * (pack ? pack : 1)));
+    }
+    if (D.nvpt && D.nc) {
+      if (D.nchunks) ba_schur_cam_kernel<<<(D.nchunks + BA_SC_BLOCK / 32 - 1) / (BA_SC_BLOCK / 32), BA_SC_BLOCK, 0, st>>>(D);
+      if (D.nchunks_off && !D.intr_by_pt) ba_cam_offdiag_kernel<true><<<(D.nchunks_off + BA_SC_BLOCK / 32 - 1) / (BA_SC_BLOCK / 32), BA_SC_BLOCK, 0, st>>>(D);
+      const bool schur_pt = (dkmax > 0 && D.intr_by_pt) || D.pose_by_pt;
+      if (schur_pt) ba_schur_pt_kernel<<<gp_blocks(), 256, 0, st>>>(D);
+      launches += 1 + (schur_pt ? 1 : 0);
+    }
+    mark(PF_DAMP_SCHUR);
+    red.begin();
+    BA_CUDA(red(D.rhs, D.nc, ncclDouble, ncclSum));
+    BA_CUDA(red(D.Mbb, pack, ncclDouble, ncclSum));
+    BA_CUDA(red(d_fail, 1, ncclInt32, ncclMax));
+    BA_CUDA(red.end());
+    mark(PF_AR_SCHUR);
+    BA_TRY(checkpoint("damp + schur_cam / schur_pt"));
+    if (D.nblk && D.nc) { if (D.wide) ba_invert_blocks_kernel<BA_MAXCB><<<(D.nc + 127) / 128, 128, 0, st>>>(D); else ba_invert_blocks_kernel<6><<<(D.nc + 127) / 128, 128, 0, st>>>(D); }
+    launches += 4;
+    mark(PF_INVERT);
+    return checkpoint("invert_blocks");
+  }
+  // The reduced camera system: dense Cholesky, or PCG in batches of 8 iterations with one host round trip per batch.
+  // *h is current afterwards when read is set (the PCG always reads it back).
+  int linear_solve(const double& cost, bool read) {
+    BA_CUDA(zero(D.ctl, offsetof(BaCtl, iters_total)));  // keeps iters_total
+    BA_CUDA(cudaMemcpyAsync(&D.ctl->cost, &cost, sizeof(double), cudaMemcpyHostToDevice, st));
+    if (!D.nc || path.dense) {
+      if (D.nc) { BA_DISPATCH_DC(ba_launch_dense, D, st); launches += 3; }
+      if (read) BA_CUDA(read_ctl());
+      return 0;
+    }
+    ba_pcg_init_kernel<<<gc_blocks(), 256, 0, st>>>(D);
+    ++launches;
+    mark(PF_PCG_INIT);
+    const int zero_q = replica() ? 1 : 0;   // D_c^2 p is contributed by rank 0 only
+    auto mid = [&](int do_post) {
+      if (path.mid_staged) ba_pcg_mid_staged_kernel<<<1, BA_PCG_T, path.mid_staged, st>>>(D, o->eta, path.r_tol, path.max_cg, zero_q, do_post);
+      else ba_pcg_mid_kernel<<<1, BA_PCG_T, path.mid_smem, st>>>(D, o->eta, path.r_tol, path.max_cg, zero_q, do_post, path.mid_smem ? 1 : 0);
+    };
+    if (path.fused_pcg) { mid(0); ++launches; }
+    for (int issued = 0;;) {
+      const int batch = std::min(8, path.max_cg - issued);
+      for (int b = 0; b < batch; ++b) {
+        if (!path.fused_pcg) {
+          ba_pcg_precond_kernel<<<gc_blocks(), 256, 0, st>>>(D);
+          ba_pcg_direction_kernel<<<gc_blocks(), 256, 0, st>>>(D);
+          if (zero_q) BA_CUDA(zero(D.q, sizeof(double) * D.nc));
+        }
+        if (b == 0) BA_CUDA(cudaEventRecord(ev[2], st));  // first SpMV of a batch always does real work
+        BA_DISPATCH_DC(ba_launch_spmv, D, path, st);
+        if (b == 0) BA_CUDA(cudaEventRecord(ev[3], st));
+        mark(PF_SPMV);
+        BA_CUDA(red(D.q, D.nc, ncclDouble, ncclSum, &D.ctl->done));  // the one data-path collective of a PCG iteration
+        mark(PF_AR_Q);
+        if (path.fused_pcg) {
+          mid(1);
+          launches += 3;
+          mark(PF_MID);
+        } else {
+          ba_pcg_dot_pq_kernel<<<gc_blocks(), 256, 0, st>>>(D);
+          ba_pcg_update_kernel<<<gc_blocks(), 256, 0, st>>>(D);
+          ba_pcg_step_kernel<<<1, 1, 0, st>>>(D, o->eta, path.r_tol, path.max_cg);
+          launches += 7;
+        }
+      }
+      issued += batch;
+      BA_CUDA(read_ctl());
+      mark(PF_HOST);
+      if (batch > 0) { float ms = 0; cudaEventElapsedTime(&ms, ev[2], ev[3]); spmv_ms += ms; spmv_launches += 1; }
+      if (h->done || issued >= path.max_cg) return 0;
+    }
+  }
+  // the candidate: point steps by back-substitution, the parameter update, its cost and the model decrease, read back
+  int evaluate_step() {
+    BA_CUDA(zero(&D.ctl->model));
+    BA_DISPATCH_DC(ba_launch_backsub, D, st);
+    mark(PF_BACKSUB);
+    BA_TRY(checkpoint("backsub"));
+    { const long long n = (((long long)D.nposes + 31) & ~31LL) + (((long long)D.ncams + 31) & ~31LL) + D.npts; ba_update_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(D); }
+    BA_CUDA(zero(&D.ctl->new_cost));
+    BA_CUDA(zero(&D.ctl->cost_delta));
+    if (D.wide) ba_cost_kernel<true><<<D.nblocks, BA_BLOCK, 0, st>>>(D, D.nposes_, D.ncams_, D.npts_, D.nsensors_, &D.ctl->new_cost);
+    else ba_cost_kernel<false><<<D.nblocks, BA_BLOCK, 0, st>>>(D, D.nposes_, D.ncams_, D.npts_, D.nsensors_, &D.ctl->new_cost);
+    BA_TRY(checkpoint("update + cost"));
+    mark(PF_UPDATE_COST);
+    BA_CUDA(red(&D.ctl->new_cost, 3, ncclDouble, ncclSum));   // new_cost, model, cost_delta are adjacent in BaCtl
+    mark(PF_AR_COST);
+    launches += 3;
+    BA_CUDA(read_ctl());
+    mark(PF_HOST);
+    return 0;
+  }
+};
+// Copies the variable blocks back into the caller's arrays (constants stay bit-identical).
+static int ba_write_back(const BaLayout& L, const BaDev& D, b200ba_problem* p) {
+  const int NP = p->num_poses, NCAM = p->num_cameras, NS = p->num_sensors;
+  const long long NPT = p->num_points;
+  std::vector<double> h_poses(7 * (size_t)NP), h_cams(L.ncamparams), h_pts(3 * (size_t)NPT), h_sens(7 * (size_t)NS);
+  BA_CUDA(cudaMemcpy(h_poses.data(), D.poses, sizeof(double) * h_poses.size(), cudaMemcpyDeviceToHost));
+  BA_CUDA(cudaMemcpy(h_cams.data(), D.cams, sizeof(double) * h_cams.size(), cudaMemcpyDeviceToHost));
+  BA_CUDA(cudaMemcpy(h_pts.data(), D.pts, sizeof(double) * h_pts.size(), cudaMemcpyDeviceToHost));
+  for (int i = 0; i < NP; ++i) if (L.pose_off[i] >= 0) memcpy(p->poses + 7 * (size_t)i, h_poses.data() + 7 * (size_t)i, 56);
+  for (int c = 0; c < NCAM; ++c) for (int k = 0; k < L.cam_nvar[c]; ++k) { const int idx = L.cam_poff[c] + L.cam_var[BA_MAXP * (size_t)c + k]; p->camera_params[idx] = h_cams[idx]; }
+  if (NS) {
+    BA_CUDA(cudaMemcpy(h_sens.data(), D.sensors, sizeof(double) * h_sens.size(), cudaMemcpyDeviceToHost));
+    for (int k = 0; k < NS; ++k) if (L.sens_cam[k] >= 0 && L.cam_ns[L.sens_cam[k]]) memcpy(p->sensor_from_rig + 7 * (size_t)k, h_sens.data() + 7 * (size_t)k, 56);
+  }
+  for (long long i = 0; i < NPT; ++i) if (L.pt_var[i] >= 0) memcpy(p->points + 3 * i, h_pts.data() + 3 * i, 24);
+  return 0;
+}
+static int ba_solve_impl(const b200ba_options* o, b200ba_problem* p, b200ba_summary* sum, b200ba_comm* comm) {
+  if (!o || !p || !sum) return ba_fail(-1, "null argument");
+  memset(sum, 0, sizeof(*sum));
+  sum->termination_type = B200BA_FAILURE;
+  BaPool pool;
+  const auto t_setup0 = std::chrono::steady_clock::now();
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return ba_fail(-101, "no CUDA device: colmap_b200 has no CPU fallback");
+  if (o->gpu_index >= 0) {
+    if (o->gpu_index >= ndev) return ba_fail(-101, "gpu_index out of range");
+    cudaSetDevice(o->gpu_index);
+  }
+  BaSolve S;
+  BA_CUDA(cudaStreamCreateWithFlags(&S.st, cudaStreamNonBlocking));
+  S.o = o;
+  BaReducer& red = S.red;
+  red.comm = comm && comm->world > 1 ? comm : nullptr; red.st = S.st; red.pool = &pool; red.sms = ba_sm_count();
+  BaLayout L;
+  BA_TRY(ba_flatten(o, p, red.comm ? &red : nullptr, L, sum));
+  if (L.nothing_to_solve) { sum->termination_type = B200BA_CONVERGENCE; return 0; }
+  S.pack = L.pack; S.dkmax = L.dkmax;
+  BA_TRY(ba_select_path(o, L, red.comm != nullptr, red.sms, S.path));
+  BA_TRY(ba_upload(L, o, p, S.path, red.comm, pool, S.st, S.D));
+  sum->setup_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_setup0).count();
+
+  for (int i = 0; i < 4; ++i) BA_CUDA(cudaEventCreate(&S.ev[i]));
   // the control block is read back into pinned memory (a pageable destination makes the copy a staged, slower one)
   static thread_local BaCtl* h_pinned = nullptr;
   if (!h_pinned && cudaHostAlloc((void**)&h_pinned, sizeof(BaCtl), cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); h_pinned = nullptr; }
-  BaCtl h_pageable;
-  BaCtl& h = h_pinned ? *h_pinned : h_pageable;
-  auto read_ctl = [&]() -> cudaError_t { cudaError_t e = cudaMemcpyAsync(&h, D.ctl, sizeof(BaCtl), cudaMemcpyDeviceToHost, st); if (e != cudaSuccess) return e; return cudaStreamSynchronize(st); };
-  auto zero_field = [&](double* field) { return cudaMemsetAsync(field, 0, sizeof(double), st); };
-  // B200BA_PROFILE=1: device-timeline breakdown of the solve by phase (events between the launches; the interval that
-  // ends at a "host" mark is GPU idle time spent waiting for the host round trip).  Diagnostic only.
-  enum { PF_LIN, PF_BUILD, PF_AR_BUILD, PF_DIAG, PF_DAMP_SCHUR, PF_AR_SCHUR, PF_INVERT, PF_PCG_INIT, PF_SPMV, PF_AR_Q, PF_MID,
-         PF_HOST, PF_BACKSUB, PF_UPDATE_COST, PF_AR_COST, PF_N };
-  static const char* const pf_names[PF_N] = {"linearize", "build (cam blocks, gradient)", "all-reduce gc+Hbb", "diag/build_pt/gradmax(+AR)",
-      "damp + schur_cam", "all-reduce rhs+Mbb", "invert blocks", "pcg init", "spmv (both passes)", "all-reduce q", "pcg mid",
-      "host round trip (GPU idle)", "backsub", "update + cost", "all-reduce cost"};
-  const bool prof_on = getenv("B200BA_PROFILE") != nullptr;
-  std::vector<cudaEvent_t> pf_ev; std::vector<int> pf_tag;
-  auto mark = [&](int tag) { if (!prof_on) return; cudaEvent_t e; if (cudaEventCreate(&e) != cudaSuccess) return; cudaEventRecord(e, st); pf_ev.push_back(e); pf_tag.push_back(tag); };
-  auto linearize_current = [&](int apply_scale) {
-    zero_field(&D.ctl->cost);
-    ba_launch_linearize(D, apply_scale, st);
-    mark(PF_LIN);
-    allreduce(&D.ctl->cost, 1, ncclDouble, ncclSum);
-    mark(PF_AR_COST);
-    launches += 2;
-  };
-
-  const bool dbg = getenv("B200BA_CHECK") != nullptr;   // diagnostic: synchronise and test for asynchronous errors after every group of launches
-#define BA_CHECKPOINT(label)                                                                                   \
-  do { if (dbg) { cudaError_t e__ = cudaStreamSynchronize(st); if (e__ == cudaSuccess) e__ = cudaGetLastError(); \
-       if (e__ != cudaSuccess) return ba_fail(-100, std::string("checkpoint ") + label + ": " + cudaGetErrorString(e__)); } } while (0)
-  BA_CUDA(cudaEventRecord(ev0, st));
-  // iteration 0: Jacobian, jacobi scaling
-  linearize_current(0);
-  BA_CHECKPOINT("linearize(0)");
-  BA_CUDA(cudaMemsetAsync(D.scale_c, 0, sizeof(double) * (nc ? nc : 1), st));
-  BA_CUDA(cudaMemsetAsync(D.scale_p, 0, sizeof(double) * (nvpt ? 3 * (size_t)nvpt : 1), st));
-  ba_colnorm_kernel<<<nblocks, BA_BLOCK, 0, st>>>(D);
-  BA_CUDA(allreduce(D.scale_c, nc, ncclDouble, ncclSum));
-  if (nc) ba_make_scale_kernel<<<gc_blocks, 256, 0, st>>>(D.scale_c, nc, o->jacobi_scaling);
-  if (nvpt) ba_make_scale_kernel<<<(3 * nvpt + 255) / 256, 256, 0, st>>>(D.scale_p, 3LL * nvpt, o->jacobi_scaling);
-  launches += 3;
-  BA_CHECKPOINT("colnorm");
-  linearize_current(1);  // store the scaled Jacobian (fp32) in both orders
-  BA_CHECKPOINT("linearize(1)");
-  BA_CUDA(read_ctl());
+  S.h = h_pinned ? h_pinned : &S.h_pageable;
+  const BaCtl& h = *S.h;
+  BA_CUDA(cudaEventRecord(S.ev[0], S.st));
+  BA_TRY(S.linearize_scaled());
+  BA_CUDA(S.read_ctl());
   double cost = h.cost;
   sum->initial_cost = cost;
-  double radius = o->initial_trust_region_radius, decrease_factor = 2.0;
-  int iter = 0;
+  double radius = o->initial_trust_region_radius, decrease_factor = 2.0, last_gmax = 0.0;
+  int iter = 0, discarded_pcg = 0;
   sum->termination_type = B200BA_NO_CONVERGENCE;
-  const bool exact = (lst != B200BA_ITERATIVE_SCHUR);
-  // exact reduced solves (DENSE_/SPARSE_SCHUR) are obtained by running the same PCG to a 1e-12 relative residual
-  const double q_tol = o->eta, r_tol = exact ? 1e-12 : -1.0;
-  const int max_cg = exact ? std::max(10 * nc + 100, o->max_linear_solver_iterations) : o->max_linear_solver_iterations;
   bool finished = false;
   const bool verbose = getenv("B200BA_VERBOSE") != nullptr;
-  const bool fused_pcg = nc <= BA_PCG_FUSED_MAX && getenv("B200BA_PCG_MULTI") == nullptr;
-  // r of ba_pcg_mid_kernel in (at most 160 KB of) shared memory; tests/test_ba_paths_gpu.py mirrors this threshold
-  const size_t mid_smem = (fused_pcg && (size_t)nc * sizeof(double) <= 160 * 1024 && getenv("B200BA_MID_GLOBAL") == nullptr) ? (size_t)nc * sizeof(double) : 0;
-  if (mid_smem) BA_CUDA(cudaFuncSetAttribute(ba_pcg_mid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-  const size_t mid_staged = (fused_pcg && nc <= BA_PCG_T * BA_MID_EPT && getenv("B200BA_MID_PLAIN") == nullptr) ? (size_t)nc * BA_MID_STAGE_BYTES_PER_ROW : 0;
-  if (mid_staged) BA_CUDA(cudaFuncSetAttribute(ba_pcg_mid_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_PCG_T * BA_MID_EPT * BA_MID_STAGE_BYTES_PER_ROW));
-  { const char* e = getenv("B200BA_SPMV_SMEM"); g_ba_spmv_smem = e ? atoi(e) != 0 : 1; }   // per solve: an unset variable restores the default
-  double last_gmax = 0.0;
-  int discarded_pcg = 0;
   while (!finished) {
-    // normal equations from the current (scaled) Jacobian
-    BA_CUDA(cudaMemsetAsync(D.gc, 0, sizeof(double) * (nc ? nc : 1), st));
-    BA_CUDA(cudaMemsetAsync(D.Hbb, 0, sizeof(double) * (pack ? pack : 1), st));
-    BA_CUDA(zero_field(&D.ctl->gmax));
-    if (D.nchunks) ba_build_cam_sorted_kernel<<<(D.nchunks + BA_SC_BLOCK / 32 - 1) / (BA_SC_BLOCK / 32), BA_SC_BLOCK, 0, st>>>(D);
-    BA_CHECKPOINT("build_cam_sorted");
-    if (D.nchunks_off) ba_cam_offdiag_kernel<false><<<(D.nchunks_off + BA_SC_BLOCK / 32 - 1) / (BA_SC_BLOCK / 32), BA_SC_BLOCK, 0, st>>>(D);
-    BA_CHECKPOINT("cam_offdiag<false>");
-    mark(PF_BUILD);
-    group_begin();
-    BA_CUDA(allreduce(D.gc, nc, ncclDouble, ncclSum));
-    BA_CUDA(allreduce(D.Hbb, pack, ncclDouble, ncclSum));
-    BA_CUDA(group_end());
-    mark(PF_AR_BUILD);
-    if (nc) ba_diag_from_blocks_kernel<<<gc_blocks, 256, 0, st>>>(D);
-    if (nvpt) ba_build_pt_kernel<<<gp_blocks, 256, 0, st>>>(D);
-    BA_CHECKPOINT("diag + build_pt");
-      { const long long n = (((long long)NP + 31) & ~31LL) + (((long long)NCAM + 31) & ~31LL) + 3LL * nvpt; ba_gradmax_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(D); }
-    BA_CHECKPOINT("gradmax");
-    launches += 4;
-    BA_CUDA(allreduce(&D.ctl->gmax, 1, ncclDouble, ncclMax));
-    mark(PF_DIAG);
+    BA_TRY(S.build());
     // The gradient-norm test of this iteration is read back together with the first linear-solve batch (one host
     // round trip less per LM iteration); if it says "converged" the enqueued solve is discarded.
-    bool check_gmax = true;
-    bool accepted = false;
+    bool check_gmax = true, accepted = false;
     while (!accepted) {
       if (iter >= o->max_num_iterations) {
-        if (check_gmax) { BA_CUDA(read_ctl()); last_gmax = h.gmax; if (h.gmax <= o->gradient_tolerance) sum->termination_type = B200BA_CONVERGENCE; }
+        if (check_gmax) { BA_CUDA(S.read_ctl()); last_gmax = h.gmax; if (h.gmax <= o->gradient_tolerance) sum->termination_type = B200BA_CONVERGENCE; }
         finished = true; break;
       }
       ++iter;
-      BA_CUDA(cudaMemsetAsync(d_fail, 0, sizeof(int), st));
-      if (nvpt) ba_damp_pt_kernel<<<gp_blocks, 256, 0, st>>>(D, 1.0 / radius, o->min_lm_diagonal, o->max_lm_diagonal, d_fail);
-      if (nc) ba_damp_cam_kernel<<<gc_blocks, 256, 0, st>>>(D, 1.0 / radius, o->min_lm_diagonal, o->max_lm_diagonal);
-      if (sharded && comm->rank != 0) {  // the replicated terms (-g_c, H_bb + D) are contributed by rank 0 only
-        BA_CUDA(cudaMemsetAsync(D.rhs, 0, sizeof(double) * (nc ? nc : 1), st));
-        BA_CUDA(cudaMemsetAsync(D.Mbb, 0, sizeof(double) * (pack ? pack : 1), st));
-      }
-      if (nvpt && nc) {
-        if (D.nchunks) ba_schur_cam_kernel<<<(D.nchunks + BA_SC_BLOCK / 32 - 1) / (BA_SC_BLOCK / 32), BA_SC_BLOCK, 0, st>>>(D);
-        if (D.nchunks_off && !intr_by_pt) ba_cam_offdiag_kernel<true><<<(D.nchunks_off + BA_SC_BLOCK / 32 - 1) / (BA_SC_BLOCK / 32), BA_SC_BLOCK, 0, st>>>(D);
-        const bool schur_pt = (dkmax > 0 && intr_by_pt) || D.pose_by_pt;
-        if (schur_pt) ba_schur_pt_kernel<<<gp_blocks, 256, 0, st>>>(D);
-        launches += 1 + (schur_pt ? 1 : 0);
-      }
-      mark(PF_DAMP_SCHUR);
-      group_begin();
-      BA_CUDA(allreduce(D.rhs, nc, ncclDouble, ncclSum));
-      BA_CUDA(allreduce(D.Mbb, pack, ncclDouble, ncclSum));
-      BA_CUDA(allreduce(d_fail, 1, ncclInt32, ncclMax));
-      BA_CUDA(group_end());
-      mark(PF_AR_SCHUR);
-      BA_CHECKPOINT("damp + schur_cam / schur_pt");
-      if (nblk && nc) { if (D.wide) ba_invert_blocks_kernel<BA_MAXCB><<<(nc + 127) / 128, 128, 0, st>>>(D); else ba_invert_blocks_kernel<6><<<(nc + 127) / 128, 128, 0, st>>>(D); }
-      launches += 4;
-      mark(PF_INVERT);
-      BA_CHECKPOINT("invert_blocks");
-      // PCG
-      BA_CUDA(cudaMemsetAsync(D.ctl, 0, offsetof(BaCtl, iters_total), st));  // keeps iters_total
-      BA_CUDA(cudaMemcpyAsync(&D.ctl->cost, &cost, sizeof(double), cudaMemcpyHostToDevice, st));
-      if (nc && dense) {
-        BA_DISPATCH_DC(ba_launch_dense, D, st);
-        launches += 3;
-        if (check_gmax) BA_CUDA(read_ctl());
-      } else if (nc) {
-        ba_pcg_init_kernel<<<gc_blocks, 256, 0, st>>>(D);
-        ++launches;
-        mark(PF_PCG_INIT);
-        int issued = 0;
-        const bool zero_q = sharded && comm->rank != 0;   // D_c^2 p is contributed by rank 0 only
-        if (fused_pcg) { if (mid_staged) ba_pcg_mid_staged_kernel<<<1, BA_PCG_T, mid_staged, st>>>(D, q_tol, r_tol, max_cg, zero_q ? 1 : 0, 0); else ba_pcg_mid_kernel<<<1, BA_PCG_T, mid_smem, st>>>(D, q_tol, r_tol, max_cg, zero_q ? 1 : 0, 0, mid_smem ? 1 : 0); ++launches; }
-        for (;;) {
-          const int batch = std::min(8, max_cg - issued);
-          for (int b = 0; b < batch; ++b) {
-            if (!fused_pcg) {
-              ba_pcg_precond_kernel<<<gc_blocks, 256, 0, st>>>(D);
-              ba_pcg_direction_kernel<<<gc_blocks, 256, 0, st>>>(D);
-              if (zero_q) BA_CUDA(cudaMemsetAsync(D.q, 0, sizeof(double) * nc, st));
-            }
-            if (b == 0) BA_CUDA(cudaEventRecord(evs0, st));  // first SpMV of a batch always does real work
-            BA_DISPATCH_DC(ba_launch_spmv, D, st);
-            if (b == 0) BA_CUDA(cudaEventRecord(evs1, st));
-            mark(PF_SPMV);
-            BA_CUDA(allreduce_if(D.q, nc, ncclDouble, ncclSum, &D.ctl->done));  // the one data-path collective of a PCG iteration
-            mark(PF_AR_Q);
-            if (fused_pcg) {
-              if (mid_staged) ba_pcg_mid_staged_kernel<<<1, BA_PCG_T, mid_staged, st>>>(D, q_tol, r_tol, max_cg, zero_q ? 1 : 0, 1);
-              else ba_pcg_mid_kernel<<<1, BA_PCG_T, mid_smem, st>>>(D, q_tol, r_tol, max_cg, zero_q ? 1 : 0, 1, mid_smem ? 1 : 0);
-              launches += 3;
-              mark(PF_MID);
-            } else {
-              ba_pcg_dot_pq_kernel<<<gc_blocks, 256, 0, st>>>(D);
-              ba_pcg_update_kernel<<<gc_blocks, 256, 0, st>>>(D);
-              ba_pcg_step_kernel<<<1, 1, 0, st>>>(D, q_tol, r_tol, max_cg);
-              launches += 7;
-            }
-          }
-          issued += batch;
-          BA_CUDA(read_ctl());
-          mark(PF_HOST);
-          if (batch > 0) { float ms = 0; cudaEventElapsedTime(&ms, evs0, evs1); spmv_ms += ms; spmv_launches += 1; }
-          if (h.done || issued >= max_cg) break;
-        }
-      }
+      BA_TRY(S.damp(radius));
+      BA_TRY(S.linear_solve(cost, check_gmax));
       if (check_gmax) {
         check_gmax = false;
-        if (!nc) BA_CUDA(read_ctl());
         last_gmax = h.gmax;
         if (h.gmax <= o->gradient_tolerance) {
-          --iter; discarded_pcg = nc ? h.it : 0;
+          --iter; discarded_pcg = L.nc ? h.it : 0;
           sum->termination_type = B200BA_CONVERGENCE; finished = true; break;
         }
       }
-      BA_CHECKPOINT("linear solve");
-      BA_CUDA(zero_field(&D.ctl->model));
-      BA_DISPATCH_DC(ba_launch_backsub, D, st);
-      mark(PF_BACKSUB);
-      BA_CHECKPOINT("backsub");
-      { const long long n = (((long long)NP + 31) & ~31LL) + (((long long)NCAM + 31) & ~31LL) + NPT; ba_update_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(D); }
-      BA_CUDA(zero_field(&D.ctl->new_cost));
-      BA_CUDA(zero_field(&D.ctl->cost_delta));
-      if (D.wide) ba_cost_kernel<true><<<nblocks, BA_BLOCK, 0, st>>>(D, D.nposes_, D.ncams_, D.npts_, D.nsensors_, &D.ctl->new_cost);
-      else ba_cost_kernel<false><<<nblocks, BA_BLOCK, 0, st>>>(D, D.nposes_, D.ncams_, D.npts_, D.nsensors_, &D.ctl->new_cost);
-      BA_CHECKPOINT("update + cost");
-      mark(PF_UPDATE_COST);
-      BA_CUDA(allreduce(&D.ctl->new_cost, 3, ncclDouble, ncclSum));   // new_cost, model, cost_delta are adjacent in BaCtl
-      mark(PF_AR_COST);
-      launches += 3;
-      BA_CUDA(read_ctl());
-      mark(PF_HOST);
+      BA_TRY(S.checkpoint("linear solve"));
+      BA_TRY(S.evaluate_step());
       const int failed = h.fail;
       const double model = h.model, new_cost = h.new_cost;
       // cost change summed residual by residual (same quantity as cost - new_cost, without the cancellation)
-      const double cost_change_acc = -h.cost_delta;
-      const double rho_q = (!failed && model > 0) ? cost_change_acc / model : 0.0;
+      const double cost_change = -h.cost_delta;
+      const double rho_q = (!failed && model > 0) ? cost_change / model : 0.0;
       if (verbose) fprintf(stderr, "[b200ba] it %d cost %.12g new %.12g model %.6g rho %.6g radius %.4g pcg_it %d (total %d) gmax %.4g failed %d\n",
                            iter, cost, new_cost, model, rho_q, radius, h.it, h.iters_total, last_gmax, failed);
       if (!failed && model > 0 && rho_q > o->min_relative_decrease) {
         accepted = true;
         sum->num_successful_steps++;
-        std::swap(D.poses, D.nposes_); std::swap(D.cams, D.ncams_); std::swap(D.pts, D.npts_); std::swap(D.sensors, D.nsensors_);
-        const double cost_change = cost_change_acc;
-        linearize_current(1);
+        std::swap(S.D.poses, S.D.nposes_); std::swap(S.D.cams, S.D.ncams_); std::swap(S.D.pts, S.D.npts_); std::swap(S.D.sensors, S.D.nsensors_);
+        BA_TRY(S.linearize(1));
         // the cost at the accepted point is the candidate cost just evaluated: no third host round trip per LM iteration
         // (the re-linearisation sums the same per-observation values; it only differs in the order of the block sums)
         cost = new_cost;
@@ -3376,43 +3426,23 @@ static int ba_solve_impl(const b200ba_options* o, b200ba_problem* p, b200ba_summ
       }
     }
   }
-  BA_CUDA(cudaEventRecord(ev1, st));
-  BA_CUDA(read_ctl());
+  BA_CUDA(cudaEventRecord(S.ev[1], S.st));
+  BA_CUDA(S.read_ctl());
   float solve_ms = 0;
-  BA_CUDA(cudaEventElapsedTime(&solve_ms, ev0, ev1));
+  BA_CUDA(cudaEventElapsedTime(&solve_ms, S.ev[0], S.ev[1]));
   sum->solve_ms = solve_ms;
-  if (prof_on) {
-    double acc[PF_N] = {0}; int cnt[PF_N] = {0};
-    for (size_t k = 1; k < pf_ev.size(); ++k) { float ms = 0; if (cudaEventElapsedTime(&ms, pf_ev[k - 1], pf_ev[k]) == cudaSuccess) { acc[pf_tag[k]] += ms; cnt[pf_tag[k]]++; } }
-    for (cudaEvent_t e : pf_ev) cudaEventDestroy(e);
-    if (!sharded || comm->rank == 0) {
-      const int lm = sum->num_successful_steps + sum->num_unsuccessful_steps;
-      fprintf(stderr, "[b200ba profile] world %d, %d LM iterations, %.1f ms on the device\n", sharded ? comm->world : 1, lm, solve_ms);
-      for (int t = 0; t < PF_N; ++t) if (cnt[t]) fprintf(stderr, "[b200ba profile] %-30s %8.2f ms %5.1f %%  n=%6d  %7.1f us each  %7.1f us / LM it\n", pf_names[t], acc[t], 100.0 * acc[t] / solve_ms, cnt[t], 1e3 * acc[t] / cnt[t], 1e3 * acc[t] / std::max(lm, 1));
-    }
-  }
-  if (sharded && comm->p2p.ok) {
+  if (S.profile && !S.replica()) S.report(red.comm ? red.comm->world : 1, sum->num_successful_steps + sum->num_unsuccessful_steps, solve_ms);
+  if (red.comm && red.comm->p2p.ok) {
     unsigned long long timed_out = 0;
-    BA_CUDA(cudaMemcpy(&timed_out, comm->p2p.state + 2, sizeof(timed_out), cudaMemcpyDeviceToHost));
+    BA_CUDA(cudaMemcpy(&timed_out, red.comm->p2p.state + 2, sizeof(timed_out), cudaMemcpyDeviceToHost));
     if (timed_out) return ba_fail(-111, "peer-memory all-reduce timed out waiting for a rank");
   }
   sum->final_cost = cost;
   sum->num_linear_solver_iterations = h.iters_total - discarded_pcg;
-  sum->kernel_launches = launches + p2p_launches;
-  sum->spmv_launches = spmv_launches;
-  sum->spmv_ms_total = spmv_ms;
-  // write back variable blocks only (constants stay bit-identical)
-  BA_CUDA(cudaMemcpy(h_poses.data(), D.poses, sizeof(double) * h_poses.size(), cudaMemcpyDeviceToHost));
-  BA_CUDA(cudaMemcpy(h_cams.data(), D.cams, sizeof(double) * h_cams.size(), cudaMemcpyDeviceToHost));
-  BA_CUDA(cudaMemcpy(h_pts.data(), D.pts, sizeof(double) * h_pts.size(), cudaMemcpyDeviceToHost));
-  for (int i = 0; i < NP; ++i) if (pose_off[i] >= 0) memcpy(p->poses + 7 * (size_t)i, h_poses.data() + 7 * (size_t)i, 56);
-  for (int c = 0; c < NCAM; ++c) for (int k = 0; k < cam_nvar[c]; ++k) { const int idx = cam_poff[c] + cam_var[BA_MAXP * (size_t)c + k]; p->camera_params[idx] = h_cams[idx]; }
-  if (NS) {
-    BA_CUDA(cudaMemcpy(h_sens.data(), D.sensors, sizeof(double) * h_sens.size(), cudaMemcpyDeviceToHost));
-    for (int k = 0; k < NS; ++k) if (sens_cam[k] >= 0 && cam_ns[sens_cam[k]]) memcpy(p->sensor_from_rig + 7 * (size_t)k, h_sens.data() + 7 * (size_t)k, 56);
-  }
-  for (long long i = 0; i < NPT; ++i) if (pt_var[i] >= 0) memcpy(p->points + 3 * i, h_pts.data() + 3 * i, 24);
-  return 0;   // pool, stream and events are released by their guards
+  sum->kernel_launches = S.launches + red.launches;
+  sum->spmv_launches = S.spmv_launches;
+  sum->spmv_ms_total = S.spmv_ms;
+  return ba_write_back(L, S.D, p);   // pool, stream and events are released by their guards
 }
 
 extern "C" {
@@ -3453,18 +3483,18 @@ int b200ba_test_project_wide(int model_id, const double* params, const double* u
 
 // The host flattening of b200ba_solve without a GPU: which observation sits in which slot.  Two-call pattern: with
 // capacity 0 only the sizes come back.  info[10] = {nslots, nvpt, nblocks_warp, nblocks_var, nblocks_giant0,
-// nblocks_giant1, camera-side dimension, max variable intrinsics, num_residuals, num_effective_parameters}.
+// nblocks_giant1, camera-side dimension, max variable intrinsics, num_residuals, num_effective_parameters}.  A problem
+// with nothing to solve returns 0 and leaves info as it is.
 int b200ba_test_pack(const b200ba_options* o, b200ba_problem* p, int64_t capacity, int32_t* s_obs, int32_t* s_lpt,
                      int32_t* s_seg, int32_t* vpt_s0, int32_t* vpt_s1, int32_t* vpt_point, int64_t* info) {
-  BaHostLayout L;
-  b200ba_summary sum;
-  g_ba_layout_out = &L;
-  const int rc = ba_solve_impl(o, p, &sum, nullptr);
-  g_ba_layout_out = nullptr;
-  if (rc != -102) return rc;   // -102 = "stopped after the host flattening" (the expected outcome here)
-  info[0] = (int64_t)L.s_obs.size(); info[1] = L.nvpt; info[2] = L.nblocks_warp; info[3] = L.nblocks_var;
+  if (!o || !p) return ba_fail(-1, "null argument");
+  BaLayout L;
+  b200ba_summary sum = {};
+  const int rc = ba_flatten(o, p, nullptr, L, &sum);
+  if (rc || L.nothing_to_solve) return rc;
+  info[0] = (int64_t)L.s_obs.size(); info[1] = L.nvpt; info[2] = L.nblocks_warp; info[3] = L.nblocks_giant0;
   info[4] = L.nblocks_giant0; info[5] = L.nblocks_giant1; info[6] = L.nc; info[7] = L.dkmax;
-  info[8] = L.num_residuals; info[9] = L.num_effective_parameters;
+  info[8] = sum.num_residuals; info[9] = sum.num_effective_parameters;
   if (capacity == 0) return 0;
   if (capacity < (int64_t)L.s_obs.size()) return -12;
   memcpy(s_obs, L.s_obs.data(), sizeof(int) * L.s_obs.size());
