@@ -763,24 +763,15 @@ class BundleAdjuster:
     def Options(self): return self.options_
     def Config(self): return self.config_
 
-    def Solve(self) -> BundleAdjustmentSummary:
+    def flat_problem(self):
+        """The flat problem Solve() hands to the GPU: the flattening of the reconstruction with the gauge applied.
+        Returns (flat, pose_ids, camera_ids, point_ids); pose_ids are image ids, or frame ids for reconstructions with
+        frames.  EstimateBACovariance reads the same problem."""
         rec = self.reconstruction_
         flat, image_ids, camera_ids, point_ids = flatten_reconstruction(self.options_, self.config_, rec)
+        if rec.frames:      # rigs: the flattening applied the gauge
+            return flat, image_ids, camera_ids, point_ids
         lib = _bind(load_library())
-        if rec.frames:      # rigs: the flattening applied the gauge; poses are frames, sensors the non-reference cameras
-            summary = solve_flat(self.options_, flat)
-            for k, f in enumerate(image_ids):
-                rec.frames[f].rig_from_world[:] = flat.poses[k]
-            for k, c in enumerate(flat.sensor_camera_ids):
-                for rig in rec.rigs.values():
-                    if c in rig.sensors:
-                        rig.sensors[c][:] = flat.sensors[k]
-            for k, c in enumerate(camera_ids):
-                n = MODEL_NUM_PARAMS[rec.cameras[c].model_id]
-                rec.cameras[c].params[:] = flat.cam_params[flat.cam_off[k]:flat.cam_off[k] + n]
-            for k, p in enumerate(point_ids):
-                rec.points3D[p].xyz[:] = flat.points[k]
-            return summary
         if self.config_.FixedGauge() == TWO_CAMS_FROM_WORLD and self.options_.refine_rig_from_world:
             # gauge search runs over the images of the config in ascending id (std::set<image_t>), :346-385
             co, cp = self.options_.to_c(), flat.to_c()
@@ -803,6 +794,25 @@ class BundleAdjuster:
                 flat.pose_fixed_dim[idx] = out_d
         elif self.config_.FixedGauge() == THREE_POINTS:
             fix_gauge_three_points(flat)
+        return flat, image_ids, camera_ids, point_ids
+
+    def Solve(self) -> BundleAdjustmentSummary:
+        rec = self.reconstruction_
+        flat, image_ids, camera_ids, point_ids = self.flat_problem()
+        if rec.frames:      # poses are frames, sensors the non-reference cameras
+            summary = solve_flat(self.options_, flat)
+            for k, f in enumerate(image_ids):
+                rec.frames[f].rig_from_world[:] = flat.poses[k]
+            for k, c in enumerate(flat.sensor_camera_ids):
+                for rig in rec.rigs.values():
+                    if c in rig.sensors:
+                        rig.sensors[c][:] = flat.sensors[k]
+            for k, c in enumerate(camera_ids):
+                n = MODEL_NUM_PARAMS[rec.cameras[c].model_id]
+                rec.cameras[c].params[:] = flat.cam_params[flat.cam_off[k]:flat.cam_off[k] + n]
+            for k, p in enumerate(point_ids):
+                rec.points3D[p].xyz[:] = flat.points[k]
+            return summary
         summary = solve_flat(self.options_, flat)
         # write back in place (variable blocks only changed)
         for k, i in enumerate(image_ids):
@@ -818,3 +828,236 @@ class BundleAdjuster:
 def CreateDefaultBundleAdjuster(options, config, reconstruction) -> BundleAdjuster:
     """Factory (bundle_adjustment.cc:314-336); this build has exactly one backend."""
     return BundleAdjuster(options, config, reconstruction)
+
+
+# ------------------------------------------------------------------------------------------------ covariance
+class BACovarianceOptions:
+    """BACovarianceOptions (covariance.h): for which parameters, and the damping of the point (and, in the POSES modes,
+    the intrinsics / sensor) diagonal blocks."""
+    POSES, POINTS, POSES_AND_POINTS, ALL = 0, 1, 2, 3
+
+    def __init__(self, params=3, damping=1e-8):
+        self.params, self.damping = params, damping
+
+
+class _CCovOptions(ctypes.Structure):
+    _fields_ = [("params", ctypes.c_int), ("damping", ctypes.c_double)]
+
+
+def _bind_cov(lib):
+    if getattr(lib, "_cov_bound", False):
+        return lib
+    vp, i64 = ctypes.c_void_p, ctypes.c_int64
+    lib.b200ba_estimate_covariance.argtypes = [ctypes.POINTER(_COptions), ctypes.POINTER(_CCovOptions), ctypes.POINTER(_CProblem),
+                                               ctypes.POINTER(vp)]
+    lib.b200ba_covariance_point.argtypes = [vp, i64, _f64p]
+    lib.b200ba_covariance_pose.argtypes = [vp, ctypes.c_int, _f64p]
+    lib.b200ba_covariance_pose_cross.argtypes = [vp, ctypes.c_int, ctypes.c_int, _f64p, _i32p, _i32p]
+    lib.b200ba_covariance_camera.argtypes = [vp, ctypes.c_int, _f64p]
+    lib.b200ba_covariance_sensor.argtypes = [vp, ctypes.c_int, _f64p]
+    lib.b200ba_covariance_poses_all.argtypes = [vp, _f64p, _i8p]
+    lib.b200ba_covariance_points_all.argtypes = [vp, _f64p, _u8p]
+    lib.b200ba_covariance_info.argtypes = [vp, _f64p]
+    lib.b200ba_covariance_free.argtypes = [vp]
+    lib.b200ba_covariance_free.restype = None
+    lib._cov_bound = True
+    return lib
+
+
+class FlatCovariance:
+    """b200ba_covariance over flat indices (pose, camera, sensor, point index of the FlatProblem).  Every getter returns
+    None where the reference returns nullopt.  close() (or garbage collection) frees the device memory."""
+
+    def __init__(self, lib, handle, num_poses, num_points):
+        self._lib, self._h, self.num_poses, self.num_points = lib, handle, num_poses, num_points
+
+    def __del__(self):
+        self.close()
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.b200ba_covariance_free(self._h)
+            self._h = None
+
+    def _square(self, fn, idx, cap):
+        buf = np.zeros(cap)
+        n = fn(self._h, idx, buf.ctypes.data_as(_f64p))
+        return buf[:n * n].reshape(n, n).copy() if n else None
+
+    def point(self, k):
+        return self._square(self._lib.b200ba_covariance_point, int(k), 9)
+
+    def pose(self, i):
+        return self._square(self._lib.b200ba_covariance_pose, int(i), 36)
+
+    def camera(self, c):
+        return self._square(self._lib.b200ba_covariance_camera, int(c), 256)
+
+    def sensor(self, s):
+        return self._square(self._lib.b200ba_covariance_sensor, int(s), 36)
+
+    def pose_cross(self, i, j):
+        buf, r, c = np.zeros(36), ctypes.c_int32(), ctypes.c_int32()
+        n = self._lib.b200ba_covariance_pose_cross(self._h, int(i), int(j), buf.ctypes.data_as(_f64p), ctypes.byref(r), ctypes.byref(c))
+        return buf[:n].reshape(r.value, c.value).copy() if n else None
+
+    def poses_all(self):
+        """(out[num_poses, 6, 6], size[num_poses]): block i is out[i, :size[i], :size[i]]."""
+        out, size = np.zeros((self.num_poses, 36)), np.zeros(self.num_poses, np.int8)
+        rc = self._lib.b200ba_covariance_poses_all(self._h, out.ctypes.data_as(_f64p), size.ctypes.data_as(_i8p))
+        if rc:
+            raise BundleAdjustmentError(f"b200ba_covariance_poses_all failed ({rc}): {self._lib.b200ba_last_error().decode()}")
+        blocks = np.zeros((self.num_poses, 6, 6))
+        for i in np.nonzero(size)[0]:
+            n = int(size[i])
+            blocks[i, :n, :n] = out[i, :n * n].reshape(n, n)
+        return blocks, size
+
+    def points_all(self):
+        """(out[num_points, 3, 3], valid[num_points])."""
+        out, valid = np.zeros((self.num_points, 9)), np.zeros(self.num_points, np.uint8)
+        rc = self._lib.b200ba_covariance_points_all(self._h, out.ctypes.data_as(_f64p), valid.ctypes.data_as(_u8p))
+        if rc:
+            raise BundleAdjustmentError(f"b200ba_covariance_points_all failed ({rc}): {self._lib.b200ba_last_error().decode()}")
+        return out.reshape(-1, 3, 3), valid
+
+    def info(self):
+        """(dimension of the factorised matrix, {phase: device ms}) of the estimate."""
+        ms = np.zeros(4)
+        n = self._lib.b200ba_covariance_info(self._h, ms.ctypes.data_as(_f64p))
+        return n, dict(zip(("setup", "build", "factorize", "inverse"), ms.tolist()))
+
+
+class CovarianceNotEstimable(BundleAdjustmentError):
+    pass
+
+
+def estimate_covariance_flat(options: BundleAdjustmentOptions, cov_options: BACovarianceOptions, flat: FlatProblem,
+                             raise_not_estimable=False):
+    """b200ba_estimate_covariance on a flat problem (rigs included).  Returns a FlatCovariance, or None when the reduced
+    matrix is rank deficient (raise_not_estimable: raise CovarianceNotEstimable with the library's message instead)."""
+    lib = _bind_cov(_bind(load_library()))
+    co, cc, cp, h = options.to_c(), _CCovOptions(int(cov_options.params), float(cov_options.damping)), flat.to_c(), ctypes.c_void_p()
+    rc = lib.b200ba_estimate_covariance(ctypes.byref(co), ctypes.byref(cc), ctypes.byref(cp), ctypes.byref(h))
+    if rc == 1:
+        if raise_not_estimable:
+            raise CovarianceNotEstimable(lib.b200ba_last_error().decode())
+        return None
+    if rc != 0:
+        raise BundleAdjustmentError(f"b200ba_estimate_covariance failed ({rc}): {lib.b200ba_last_error().decode()}")
+    return FlatCovariance(lib, h.value, len(flat.poses), len(flat.points))
+
+
+# Rigid3d (geometry/rigid3.h) uncertainty propagation; a pose is the 7-vector qx qy qz qw tx ty tz, covariances are in the
+# left-perturbation tangent order [rotation, translation]
+def _quat_to_R(q):
+    x, y, z, w = q
+    return np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w)],
+                     [2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w)],
+                     [2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)]])
+
+
+def _cross_matrix(t):
+    return np.array([[0.0, -t[2], t[1]], [t[2], 0.0, -t[0]], [-t[1], t[0], 0.0]])
+
+
+def rigid3d_adjoint(T):
+    """Rigid3d::Adjoint: [[R, 0], [[t]x R, R]]."""
+    T = np.asarray(T, np.float64)
+    R = _quat_to_R(T[:4])
+    A = np.zeros((6, 6))
+    A[:3, :3] = R; A[3:, 3:] = R; A[3:, :3] = _cross_matrix(T[4:]) @ R
+    return A
+
+
+def rigid3d_adjoint_inverse(T):
+    """Rigid3d::AdjointInverse: [[R^T, 0], [-R^T [t]x, R^T]]."""
+    T = np.asarray(T, np.float64)
+    Rt = _quat_to_R(T[:4]).T
+    A = np.zeros((6, 6))
+    A[:3, :3] = Rt; A[3:, 3:] = Rt; A[3:, :3] = -Rt @ _cross_matrix(T[4:])
+    return A
+
+
+def rigid3d_inverse(T):
+    return _rigid_inverse(np.asarray(T, np.float64))
+
+
+def GetCovarianceForRigid3dInverse(rigid3, covar):
+    """Covariance (6 x 6) of rigid3.inverse()."""
+    Ai = rigid3d_adjoint_inverse(rigid3)
+    return Ai @ covar @ Ai.T
+
+
+def GetCovarianceForComposedRigid3d(a_from_b, covar):
+    """Covariance (6 x 6) of a_from_c = a_from_b * b_from_c from the 12 x 12 covariance of (a_from_b, b_from_c)."""
+    J = np.hstack([np.eye(6), rigid3d_adjoint(a_from_b)])
+    return J @ covar @ J.T
+
+
+def GetCovarianceForRelativeRigid3d(a_from_c, b_from_c, covar):
+    """Covariance (6 x 6) of b_from_a = b_from_c * a_from_c^-1 from the 12 x 12 covariance of (a_from_c, b_from_c)."""
+    J = np.hstack([-rigid3d_adjoint(b_from_c) @ rigid3d_adjoint_inverse(a_from_c), np.eye(6)])
+    return J @ covar @ J.T
+
+
+class BACovariance:
+    """BACovariance (covariance.h) over the ids of the reconstruction."""
+
+    def __init__(self, flat_cov: FlatCovariance, pose_index, point_index, other_index):
+        self.flat_cov = flat_cov
+        self._pose, self._point, self._other = pose_index, point_index, other_index
+
+    def GetPointCov(self, point3D_id):
+        k = self._point.get(point3D_id)
+        return None if k is None else self.flat_cov.point(k)
+
+    def GetCamCovFromWorld(self, image_id):
+        k = self._pose.get(image_id)
+        return None if k is None else self.flat_cov.pose(k)
+
+    def GetCamCrossCovFromWorld(self, image_id1, image_id2):
+        k1, k2 = self._pose.get(image_id1), self._pose.get(image_id2)
+        return None if k1 is None or k2 is None else self.flat_cov.pose_cross(k1, k2)
+
+    def GetCam2CovFromCam1(self, image_id1, cam1_from_world, image_id2, cam2_from_world):
+        """Covariance of cam2_from_cam1; None unless both poses are fully variable (6 dimensions)."""
+        cov_11, cov_22 = self.GetCamCovFromWorld(image_id1), self.GetCamCovFromWorld(image_id2)
+        if cov_11 is None or cov_22 is None or cov_11.shape[0] != 6 or cov_22.shape[0] != 6:
+            return None
+        cov_12 = self.GetCamCrossCovFromWorld(image_id1, image_id2)
+        cov = np.zeros((12, 12))
+        cov[:6, :6], cov[6:, 6:], cov[:6, 6:], cov[6:, :6] = cov_11, cov_22, cov_12, cov_12.T
+        return GetCovarianceForRelativeRigid3d(cam1_from_world, cam2_from_world, cov)
+
+    def GetOtherParamsCov(self, params):
+        """params: the array the reconstruction holds (camera.params, or rig.sensors[camera_id] for a sensor_from_rig)."""
+        for arr, kind, k in self._other:
+            if arr is params:
+                return self.flat_cov.camera(k) if kind == "camera" else self.flat_cov.sensor(k)
+        return None
+
+
+def EstimateBACovariance(options: BACovarianceOptions, reconstruction: Reconstruction, bundle_adjuster: BundleAdjuster):
+    """EstimateBACovariance (covariance.cc): the covariance of the problem `bundle_adjuster` solves, at the parameters
+    the reconstruction holds now (call it after Solve()).  None when the problem is not estimable (unfixed gauge)."""
+    rec = reconstruction
+    for image_id in rec.images:
+        if not rec.IsRefInFrame(image_id):
+            raise BundleAdjustmentError(f"image {image_id} is not the reference sensor of its frame: pose covariances of "
+                                        "non-trivial frames are not supported")
+    flat, pose_ids, camera_ids, point_ids = bundle_adjuster.flat_problem()
+    cov = estimate_covariance_flat(bundle_adjuster.Options(), options, flat)
+    if cov is None:
+        return None
+    if rec.frames:      # pose k = frame k; every image is its frame's reference sensor
+        frame_index = {f: k for k, f in enumerate(pose_ids)}
+        pose_index = {i: frame_index[im.frame_id] for i, im in rec.images.items() if im.frame_id in frame_index}
+    else:
+        pose_index = {i: k for k, i in enumerate(pose_ids)}
+    others = [(rec.cameras[c].params, "camera", k) for k, c in enumerate(camera_ids)]
+    for s, c in enumerate(getattr(flat, "sensor_camera_ids", [])):
+        for rig in rec.rigs.values():
+            if c in rig.sensors:
+                others.append((rig.sensors[c], "sensor", s))
+    return BACovariance(cov, pose_index, {p: k for k, p in enumerate(point_ids)}, others)
