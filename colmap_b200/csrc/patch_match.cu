@@ -61,6 +61,10 @@ struct PmParams {
   const float* init_depth;   // geom mode
   const float* init_normal;  // geom mode, 3 planes
   uint32_t* rng;       // [perimeter][6]
+  float2* patch_store; // [pixel][ntaps_st] {w, w * ref} of every tap in the original orientation (pm_patch_kernel);
+                       // nullptr: every consumer builds the reference patch inline (pm_build_patch)
+  float* patch_inv;    // [pixel][4] 1 / sum(w), summed in the tap order of sweep frame 0..3
+  int ntaps_st;        // taps per pixel block of patch_store: ntaps rounded up to even (16-byte aligned blocks)
   float K[4][4], invK[4][4];
 };
 
@@ -132,8 +136,10 @@ __host__ __device__ __forceinline__ int pm_border_index(int W0, int H0, int r0, 
   if (c0 == 0) return 2 * W0 + (r0 - 1);
   return 2 * W0 + (H0 - 2) + (r0 - 1);
 }
-// (float)v / 255.0f for v = 0..255, IEEE division done once on the host: the same bits as the division it replaces
-__constant__ float pm_lut255[256];
+// (float)v / 255.0f for v = 0..255, IEEE division done once on the host: the same bits as the division it replaces.
+// Every kernel that reads reference colours copies it into shared memory first (pm_load_lut): the lanes of a warp
+// index it with different bytes, which __constant__ memory would serialise.
+__device__ float pm_lut255[256];
 static void pm_upload_lut() {
   static thread_local int done_dev = -1;
   int dev = 0; cudaGetDevice(&dev);
@@ -143,9 +149,24 @@ static void pm_upload_lut() {
   cudaMemcpyToSymbol(pm_lut255, h, sizeof(h));
   done_dev = dev;
 }
-__device__ __forceinline__ float pm_ref_color(const PmParams& P, int rot, int fw, int fh, int r, int c) {
+__device__ __forceinline__ void pm_load_lut(float* lut, int tid, int nthreads) {
+  for (int i = tid; i < 256; i += nthreads) lut[i] = pm_lut255[i];
+}
+__device__ __forceinline__ float pm_ref_color(const PmParams& P, const float* lut, int rot, int fw, int fh, int r, int c) {
   if (r < 0 || c < 0 || r >= fh || c >= fw) return 0.0f;
-  return pm_lut255[P.ref_img[pm_pix0(P.W0, P.H0, rot, r, c)]];
+  return lut[P.ref_img[pm_pix0(P.W0, P.H0, rot, r, c)]];
+}
+// Tap t = (tr, tc) of sweep frame `rot` (offset (dr, dc) = (-radius + step * tr, -radius + step * tc)) is the tap of
+// the original orientation at the offset the frame map rotates (dr, dc) to: (dc, -dr), (-dr, -dc), (-dc, dr) for
+// frames 1, 2, 3.  The window is symmetric, so that offset is a tap too; this returns its index.
+__device__ __forceinline__ int pm_orig_tap(int rot, int nside, int t) {
+  const int tr = t / nside, tc = t - tr * nside, m = nside - 1;
+  switch (rot) {
+    case 0: return t;
+    case 1: return tc * nside + (m - tr);
+    case 2: return (m - tr) * nside + (m - tc);
+    default: return (m - tc) * nside + tr;
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -312,14 +333,14 @@ __device__ __forceinline__ int pm_sample_image(float cdf, float u, int N) {
 }
 
 // reference patch of one pixel: bilateral weights + weighted colours + 1/sum(w); executed by one warp.
-__device__ __forceinline__ void pm_build_patch(const PmParams& P, int rot, int fw, int fh, int row, int col, float4* patch,
-                                               int lane, float* inv_wsum_out) {
-  const float center = pm_ref_color(P, rot, fw, fh, row, col);
+__device__ __forceinline__ void pm_build_patch(const PmParams& P, const float* lut, int rot, int fw, int fh, int row, int col,
+                                               float4* patch, int lane, float* inv_wsum_out) {
+  const float center = pm_ref_color(P, lut, rot, fw, fh, row, col);
   float partial = 0.0f;
   for (int t = lane; t < P.ntaps; t += 32) {
     const float4 tp = patch[t];
     const int dc = (int)tp.z, dr = (int)tp.w;
-    const float c = pm_ref_color(P, rot, fw, fh, row + dr, col + dc);
+    const float c = pm_ref_color(P, lut, rot, fw, fh, row + dr, col + dc);
     const float bw = pm_bilateral_weight(P.spatial_norm, P.color_norm, dr, dc, center, c);
     reinterpret_cast<float2*>(&patch[t])[0] = make_float2(bw, bw * c);
     partial += bw;
@@ -335,6 +356,80 @@ __device__ __forceinline__ void pm_fill_tap_offsets(const PmParams& P, float4* p
     patch[t] = make_float4(0.0f, 0.0f, (float)(-P.radius + P.step * tc), (float)(-P.radius + P.step * tr));
   }
 }
+// per CTA: tsrc[t] = index in a stored pixel block of the tap in slot t of frame `rot`'s patch
+__device__ __forceinline__ void pm_fill_tap_src(const PmParams& P, int rot, int* tsrc, int tid, int nthreads) {
+  for (int t = tid; t < P.ntaps; t += nthreads) tsrc[t] = pm_orig_tap(rot, P.nside, t);
+}
+
+// Reference patches of every pixel, once per run, for the patch store: the {w, w * ref} pairs of all taps in the
+// original orientation, and 1 / sum(w) for each of the four sweep frames.  Frame k's tap (dr, dc) reads the original tap
+// at the rotated offset (pm_orig_tap), whose weight and colour have the same bits (the weight depends on dr^2 + dc^2 and
+// the colour difference only).  The weight sum is a rounded fp32 sum, so it is formed per frame in that frame's tap order
+// with pm_build_patch's lane split and shfl.xor tree: every consumer gets exactly what its inline build would compute.
+__global__ void __launch_bounds__(128) pm_patch_kernel(const PmParams P) {
+  extern __shared__ float smemf[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* lut = smemf;
+  int2* toff = reinterpret_cast<int2*>(smemf + 256);                  // (dr, dc) of original tap t
+  int* tmap = reinterpret_cast<int*>(toff + P.ntaps_pad);              // [3][ntaps_pad] pm_orig_tap of frames 1..3
+  float* wt = reinterpret_cast<float*>(tmap + 3 * P.ntaps_pad) + warp * P.ntaps_pad;   // this warp's pixel: tap weights
+  pm_load_lut(lut, threadIdx.x, blockDim.x);
+  for (int t = threadIdx.x; t < P.ntaps; t += blockDim.x) {
+    const int tr = t / P.nside, tc = t - tr * P.nside;
+    toff[t] = make_int2(-P.radius + P.step * tr, -P.radius + P.step * tc);
+    for (int k = 1; k < 4; ++k) tmap[(k - 1) * P.ntaps_pad + t] = pm_orig_tap(k, P.nside, t);
+  }
+  __syncthreads();
+  const int npix = P.W0 * P.H0;
+  for (int p = blockIdx.x * 4 + warp; p < npix; p += gridDim.x * 4) {
+    const int row = p / P.W0, col = p - row * P.W0;
+    const float center = pm_ref_color(P, lut, 0, P.W0, P.H0, row, col);
+    float2* blk = P.patch_store + (size_t)p * P.ntaps_st;
+    float partial0 = 0.0f;
+    for (int t = lane; t < P.ntaps; t += 32) {
+      const int2 o = toff[t];
+      const float c = pm_ref_color(P, lut, 0, P.W0, P.H0, row + o.x, col + o.y);
+      const float bw = pm_bilateral_weight(P.spatial_norm, P.color_norm, o.x, o.y, center, c);
+      blk[t] = make_float2(bw, bw * c);
+      wt[t] = bw;
+      partial0 += bw;   // frame 0: the stored order is its tap order
+    }
+    __syncwarp();
+    float partial1 = 0.0f, partial2 = 0.0f, partial3 = 0.0f;
+    for (int t = lane; t < P.ntaps; t += 32) {
+      partial1 += wt[tmap[t]];
+      partial2 += wt[tmap[P.ntaps_pad + t]];
+      partial3 += wt[tmap[2 * P.ntaps_pad + t]];
+    }
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      partial0 = partial0 + __shfl_xor_sync(0xffffffffu, partial0, o);
+      partial1 = partial1 + __shfl_xor_sync(0xffffffffu, partial1, o);
+      partial2 = partial2 + __shfl_xor_sync(0xffffffffu, partial2, o);
+      partial3 = partial3 + __shfl_xor_sync(0xffffffffu, partial3, o);
+    }
+    const float inv[4] = {1.0f / partial0, 1.0f / partial1, 1.0f / partial2, 1.0f / partial3};
+    if (lane < 4) P.patch_inv[(size_t)p * 4 + lane] = (lane == 0) ? inv[0] : ((lane == 1) ? inv[1] : ((lane == 2) ? inv[2] : inv[3]));
+    __syncwarp();
+  }
+}
+
+// Copy of pixel p's stored block into patch[t].xy in frame order (tsrc from pm_fill_tap_src): one 8-byte cp.async per
+// tap, so the copy is in flight while the issuing warp does other work.  The taps of a frame are a permutation of the
+// stored order, so every lane writes its own slot; the 121 x 8 B a warp reads are one contiguous block.
+__device__ __forceinline__ void pm_copy_patch(const PmParams& P, const int* tsrc, size_t p, float4* patch, int lane) {
+  const float2* blk = P.patch_store + p * P.ntaps_st;
+  for (int t = lane; t < P.ntaps; t += 32) {
+    const unsigned dst = (unsigned)__cvta_generic_to_shared(&patch[t]);
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"(dst), "l"(blk + tsrc[t]) : "memory");
+  }
+}
+__device__ __forceinline__ void pm_copy_scalar(float* dst_smem, const float* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"((unsigned)__cvta_generic_to_shared(dst_smem)), "l"(src)
+               : "memory");
+}
+// this thread's copies have landed (other threads see them after the next barrier)
+__device__ __forceinline__ void pm_copy_wait() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
 
 // ComputeInitialCost (patch_match_cuda.cu:863-912), pixel-parallel: one warp per pixel.
 __global__ void __launch_bounds__(128) pm_initial_cost_kernel(const PmParams P) {
@@ -342,9 +437,13 @@ __global__ void __launch_bounds__(128) pm_initial_cost_kernel(const PmParams P) 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int N = P.N;
   float* poses = reinterpret_cast<float*>(smem4 + 4 * P.ntaps_pad);
+  int* tsrc = reinterpret_cast<int*>(poses + N * PM_POSE_STRIDE);
+  float* lut = reinterpret_cast<float*>(tsrc + P.ntaps_pad);
   float4* patch = smem4 + warp * P.ntaps_pad;
   for (int i = threadIdx.x; i < N * PM_POSE_STRIDE; i += blockDim.x) poses[i] = P.poses[i];
   pm_fill_tap_offsets(P, patch, lane, 32);
+  pm_fill_tap_src(P, 0, tsrc, threadIdx.x, blockDim.x);
+  pm_load_lut(lut, threadIdx.x, blockDim.x);
   __syncthreads();
   const size_t npix = (size_t)P.W0 * P.H0;
   const int g = lane >> 3, sub = lane & 7;
@@ -352,7 +451,13 @@ __global__ void __launch_bounds__(128) pm_initial_cost_kernel(const PmParams P) 
   for (size_t p = (size_t)blockIdx.x * 4 + warp; p < npix; p += (size_t)gridDim.x * 4) {
     const int row = (int)(p / P.W0), col = (int)(p - (size_t)row * P.W0);
     float inv_wsum;
-    pm_build_patch(P, 0, P.W0, P.H0, row, col, patch, lane, &inv_wsum);
+    if (P.patch_store) {
+      pm_copy_patch(P, tsrc, p, patch, lane);
+      inv_wsum = P.patch_inv[p * 4];
+      pm_copy_wait();
+    } else {
+      pm_build_patch(P, lut, 0, P.W0, P.H0, row, col, patch, lane, &inv_wsum);
+    }
     __syncwarp();
     const float4 hy = P.hyp[p];
     const float rsum = P.ref_sum[p], rsq = P.ref_sqsum[p];
@@ -466,9 +571,13 @@ __global__ void __launch_bounds__(128, 8) pm_pixel_kernel(const PmParams P, cons
   const int rot = A.rot, N = P.N;
   const int fw = (rot & 1) ? P.H0 : P.W0, fh = (rot & 1) ? P.W0 : P.H0;
   float* poses = reinterpret_cast<float*>(smem4 + 4 * P.ntaps_pad);
+  int* tsrc = reinterpret_cast<int*>(poses + N * PM_POSE_STRIDE);
+  float* lut = reinterpret_cast<float*>(tsrc + P.ntaps_pad);
   float4* patch = smem4 + warp * P.ntaps_pad;
   for (int i = threadIdx.x; i < N * PM_POSE_STRIDE; i += blockDim.x) poses[i] = P.poses[(size_t)rot * N * PM_POSE_STRIDE + i];
   pm_fill_tap_offsets(P, patch, lane, 32);
+  pm_fill_tap_src(P, rot, tsrc, threadIdx.x, blockDim.x);
+  pm_load_lut(lut, threadIdx.x, blockDim.x);
   const float iK[4] = {P.invK[rot][0], P.invK[rot][1], P.invK[rot][2], P.invK[rot][3]};
   const float Kr[4] = {P.K[rot][0], P.K[rot][1], P.K[rot][2], P.K[rot][3]};
   __syncthreads();
@@ -486,7 +595,12 @@ __global__ void __launch_bounds__(128, 8) pm_pixel_kernel(const PmParams P, cons
     const size_t p = pm_pix0(P.W0, P.H0, rot, row, col);
     const float rowf = (float)row, colf = (float)col;
     float inv_wsum;
-    pm_build_patch(P, rot, fw, fh, row, col, patch, lane, &inv_wsum);
+    if (P.patch_store) {   // in flight while the pixel's inputs load and its priors are computed
+      pm_copy_patch(P, tsrc, p, patch, lane);
+      inv_wsum = P.patch_inv[p * 4 + rot];
+    } else {
+      pm_build_patch(P, lut, rot, fw, fh, row, col, patch, lane, &inv_wsum);
+    }
     const float4 cur4 = P.hyp[p];
     float cn0 = cur4.y, cn1 = cur4.z;
     pm_normal_to_frame(rot, cn0, cn1);
@@ -520,6 +634,7 @@ __global__ void __launch_bounds__(128, 8) pm_pixel_kernel(const PmParams P, cons
         prob = sp * pt * pi * pr;
       }
     }
+    pm_copy_wait();
     if (!PRUNE) {   // every (hypothesis, image) pair, four per round
       __syncwarp();
       const int npairs = 3 * N;
@@ -616,7 +731,9 @@ __global__ void __launch_bounds__(128, 8) pm_pixel_kernel(const PmParams P, cons
   }
 }
 
-template <int WPC, bool GEOM>
+// STORE: the patch comes from the patch store (P.patch_store set).  A template parameter, not a runtime branch, so that
+// neither variant of this register-bound (128 of 128) kernel carries the other's code.
+template <int WPC, bool GEOM, bool STORE>
 __global__ void __launch_bounds__(32 * WPC, 16 / WPC) pm_serial_kernel(const PmParams P, const PmSweepArgs A) {
   extern __shared__ float4 smem4[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -631,9 +748,22 @@ __global__ void __launch_bounds__(32 * WPC, 16 / WPC) pm_serial_kernel(const PmP
   float* hyp1 = tab1 + 32;                   // depth, normal of the propagated hypothesis
   float* fctl2 = hyp1 + 4;                   // [2][4] inv_wsum, ref_sum, ref_sqsum
   float* accb = fctl2 + 8;                   // [8][33] per-sample costs of the five hypotheses (+ three geometric costs)
+  int* tsrc = reinterpret_cast<int*>(accb + 272);
+  float* lut = reinterpret_cast<float*>(tsrc + P.ntaps_pad);
   for (int i = threadIdx.x; i < N * PM_POSE_STRIDE; i += blockDim.x) poses[i] = P.poses[(size_t)rot * N * PM_POSE_STRIDE + i];
   pm_fill_tap_offsets(P, patch2, threadIdx.x, blockDim.x);
   pm_fill_tap_offsets(P, patch2 + P.ntaps_pad, threadIdx.x, blockDim.x);
+  pm_fill_tap_src(P, rot, tsrc, threadIdx.x, blockDim.x);
+  pm_load_lut(lut, threadIdx.x, blockDim.x);
+  // with the patch store, the last warp copies row + 1's patch and scalars into the other half of the double buffer
+  // while row is processed, so nothing of the patch is left on the per-row chain
+  const bool store = STORE;
+  auto copy_row = [&](int row) {
+    const size_t p = pm_pix0(P.W0, P.H0, rot, row, col);
+    float* fc = fctl2 + 4 * (row & 1);
+    pm_copy_patch(P, tsrc, p, patch2 + (row & 1) * P.ntaps_pad, lane);
+    if (lane == 0) { pm_copy_scalar(fc, P.patch_inv + p * 4 + rot); pm_copy_scalar(fc + 1, P.ref_sum + p); pm_copy_scalar(fc + 2, P.ref_sqsum + p); }
+  };
   const float iK[4] = {P.invK[rot][0], P.invK[rot][1], P.invK[rot][2], P.invK[rot][3]};
   const float Kr[4] = {P.K[rot][0], P.K[rot][1], P.K[rot][2], P.K[rot][3]};
   const float colf = (float)col;
@@ -641,7 +771,8 @@ __global__ void __launch_bounds__(32 * WPC, 16 / WPC) pm_serial_kernel(const PmP
   const unsigned gmask = 0xffu << (8 * g);
   const unsigned full = 0xffffffffu;
   const bool img_lane = lane < N;
-  __syncthreads();
+  __syncthreads();   // tap offsets and tap map complete
+  if (store && warp == WPC - 1) copy_row(0);
 
   float fwd = 0.5f;
   float prev_d = 0.0f, prev_n0 = 0.0f, prev_n1 = 0.0f, prev_n2 = 0.0f;
@@ -682,9 +813,13 @@ __global__ void __launch_bounds__(32 * WPC, 16 / WPC) pm_serial_kernel(const PmP
     float4* patch = patch2 + (row & 1) * P.ntaps_pad;
     float* fctl = fctl2 + 4 * (row & 1);
     if (warp == WPC - 1) {
-      float inv_wsum;
-      pm_build_patch(P, rot, fw, fh, row, col, patch, lane, &inv_wsum);
-      if (lane == 0) { fctl[0] = inv_wsum; fctl[1] = P.ref_sum[p]; fctl[2] = P.ref_sqsum[p]; }
+      if (store) {
+        pm_copy_wait();
+      } else {
+        float inv_wsum;
+        pm_build_patch(P, lut, rot, fw, fh, row, col, patch, lane, &inv_wsum);
+        if (lane == 0) { fctl[0] = inv_wsum; fctl[1] = P.ref_sum[p]; fctl[2] = P.ref_sqsum[p]; }
+      }
     }
     // ---- phase A (warp 0): propagated hypothesis, sampling distribution, samples
     float cost_i = 0.0f, beta_i = 0.0f, prevp_i = 0.0f, cdf = 0.0f;
@@ -711,7 +846,8 @@ __global__ void __launch_bounds__(32 * WPC, 16 / WPC) pm_serial_kernel(const PmP
       cdf = pm_cdf_lanes(prob, N, lane);
       if (lane == 0) { hyp1[0] = prev_d; hyp1[1] = prev_n0; hyp1[2] = prev_n1; hyp1[3] = prev_n2; }
     }
-    __syncthreads();  // #1: patch + propagated hypothesis visible
+    __syncthreads();  // #1: patch + propagated hypothesis visible; every warp is done with row - 1's half of the buffer
+    if (store && warp == WPC - 1 && row + 1 < fh) copy_row(row + 1);
     if (warp == 0 && row + 1 < fh) fetch_row(row + 1);
 
     // ---- phase B (all warps): NCC of the propagated hypothesis against every source image
@@ -941,15 +1077,20 @@ struct b200pm_context {
   bool dirty = false, ran = false;
   float last_ms = 0.0f, last_sweep_ms = 0.0f;
   float last_kernel_ms[3] = {0.0f, 0.0f, 0.0f};  // rand(+msg) / pixel / serial passes of the last run
+  std::vector<float> last_sweep_pass_ms;          // the same per sweep: [sweep][3]
   std::vector<cudaEvent_t> sweep_ev;
   int last_launches = 0;
   std::vector<int> src_image_idxs;
-  size_t smem_init = 0, smem_serial = 0;
+  size_t smem_init = 0, smem_serial = 0, smem_patch = 0;
+  size_t patch_store_bytes = 0;   // 0: the reference patches are built inline by every consumer
   float4* rand_hyp = nullptr; unsigned char* ntrials = nullptr; float* usamp = nullptr; float* prior3 = nullptr; float* tab3 = nullptr; float* gtab2 = nullptr;
   float* fwd_pred = nullptr;
 };
 // pixels a pixel-pass warp handles before its CTA retires (4 measured fastest on the H100; 8 was ~7 ms per C2 run slower)
 #define PM_PIXELS_PER_WARP 4
+// Device memory the patch store may take (DESIGN.md §2): 2.06 GB at 1920x1080 with window 11; 4K frames (8.2 GB) and
+// large windows (13.5 KB per pixel at radius 20) stay on the inline patch build.
+#define PM_PATCH_STORE_BUDGET (3ull << 30)
 
 template <typename T>
 static cudaError_t pm_alloc(b200pm_context* c, T** p, size_t count) {
@@ -1101,7 +1242,10 @@ int b200pm_create(const b200pm_options* o, const b200pm_problem* p, b200pm_handl
   // automatic choice depends on the column count against the SM count, so small problems never reach WPC = 1 without
   // it); B200PM_PRUNE / B200PM_PRUNE_FROM select the pixel pass's early-out schedule (PRUNE=2 evaluates nothing there,
   // which shows the serial pass does not depend on the prediction); B200PM_MAX_SWEEPS (read per run by b200pm_run)
-  // stops a run after that many sweeps, for sweep-by-sweep comparison with the oracle.
+  // stops a run after that many sweeps, for sweep-by-sweep comparison with the oracle.  B200PM_PATCH_STORE=0 keeps the
+  // inline reference-patch build even where the patch store fits its budget.
+  bool patch_store = true;
+  if (const char* e = getenv("B200PM_PATCH_STORE")) patch_store = atoi(e) != 0;
   if (const char* e = getenv("B200PM_PRUNE")) c->prune = atoi(e);
   if (const char* e = getenv("B200PM_PRUNE_FROM")) c->prune_from = atoi(e);
   if (const char* e = getenv("B200PM_WPC")) { c->wpc = atoi(e); c->wpc_auto = false; }
@@ -1115,6 +1259,7 @@ int b200pm_create(const b200pm_options* o, const b200pm_problem* p, b200pm_handl
   P.nside = (2 * P.radius) / P.step + 1;
   P.ntaps = P.nside * P.nside;
   P.ntaps_pad = (P.ntaps + 7) & ~7;
+  P.ntaps_st = (P.ntaps + 1) & ~1;
   P.num_samples = o->num_samples;
   P.geom = o->geom_consistency ? 1 : 0;
   P.filter_min_num_consistent = o->filter_min_num_consistent;
@@ -1201,8 +1346,16 @@ int b200pm_create(const b200pm_options* o, const b200pm_problem* p, b200pm_handl
     pm_prefilter_kernel<<<grd, blk, 0, s>>>(P);
     pm_init_kernel<<<grd, blk, 0, s>>>(P, c->sel[1]);
   }
-  c->smem_init = sizeof(float4) * 4 * P.ntaps_pad + sizeof(float) * (size_t)N * PM_POSE_STRIDE;
-  c->smem_serial = sizeof(float4) * 2 * P.ntaps_pad + sizeof(float) * ((size_t)N * PM_POSE_STRIDE + 32 + 4 + 8 + 272);
+  // patches, poses, then the tap map (pm_fill_tap_src) and the /255 table
+  c->smem_init = sizeof(float4) * 4 * P.ntaps_pad + sizeof(float) * ((size_t)N * PM_POSE_STRIDE + P.ntaps_pad + 256);
+  c->smem_serial = sizeof(float4) * 2 * P.ntaps_pad + sizeof(float) * ((size_t)N * PM_POSE_STRIDE + 32 + 4 + 8 + 272 + P.ntaps_pad + 256);
+  c->smem_patch = sizeof(float) * (256 + 9 * (size_t)P.ntaps_pad);   // lut, tap offsets (int2), 3 tap maps, 4 warps' weights
+  const size_t store_bytes = n * ((size_t)P.ntaps_st * sizeof(float2) + 4 * sizeof(float));
+  if (patch_store && store_bytes <= PM_PATCH_STORE_BUDGET) {
+    PM_CUDA(pm_alloc(c, &P.patch_store, n * P.ntaps_st));
+    PM_CUDA(pm_alloc(c, &P.patch_inv, 4 * n));
+    c->patch_store_bytes = store_bytes;
+  }
   PM_CUDA(pm_alloc(c, &c->rand_hyp, n));
   PM_CUDA(pm_alloc(c, &c->ntrials, n));
   PM_CUDA(pm_alloc(c, &c->usamp, n * (size_t)o->num_samples));
@@ -1218,16 +1371,21 @@ int b200pm_create(const b200pm_options* o, const b200pm_problem* p, b200pm_handl
 
 }  // extern "C"
 
-template <int WPC>
-static void pm_launch_serial(b200pm_context* c, const PmSweepArgs& A, int fw) {
+template <int WPC, bool STORE>
+static void pm_launch_serial_store(b200pm_context* c, const PmSweepArgs& A, int fw) {
   if (c->smem_serial > 48 * 1024) {
-    cudaFuncSetAttribute(pm_serial_kernel<WPC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_serial);
-    cudaFuncSetAttribute(pm_serial_kernel<WPC, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_serial);
+    cudaFuncSetAttribute(pm_serial_kernel<WPC, true, STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_serial);
+    cudaFuncSetAttribute(pm_serial_kernel<WPC, false, STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_serial);
   }
   if (c->P.geom)
-    pm_serial_kernel<WPC, true><<<fw, 32 * WPC, c->smem_serial, c->stream>>>(c->P, A);
+    pm_serial_kernel<WPC, true, STORE><<<fw, 32 * WPC, c->smem_serial, c->stream>>>(c->P, A);
   else
-    pm_serial_kernel<WPC, false><<<fw, 32 * WPC, c->smem_serial, c->stream>>>(c->P, A);
+    pm_serial_kernel<WPC, false, STORE><<<fw, 32 * WPC, c->smem_serial, c->stream>>>(c->P, A);
+}
+template <int WPC>
+static void pm_launch_serial(b200pm_context* c, const PmSweepArgs& A, int fw) {
+  if (c->P.patch_store) pm_launch_serial_store<WPC, true>(c, A, fw);
+  else pm_launch_serial_store<WPC, false>(c, A, fw);
 }
 
 extern "C" {
@@ -1238,6 +1396,8 @@ int b200pm_run(b200pm_handle c) {
   PM_CUDA(cudaSetDevice(c->device));
   const PmParams& P = c->P;
   cudaStream_t s = c->stream;
+  if (c->smem_patch > 48 * 1024)
+    PM_CUDA(cudaFuncSetAttribute(pm_patch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_patch));
   if (c->smem_init > 48 * 1024) {
     PM_CUDA(cudaFuncSetAttribute(pm_initial_cost_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_init));
     PM_CUDA(cudaFuncSetAttribute(pm_pixel_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_init));
@@ -1256,6 +1416,10 @@ int b200pm_run(b200pm_handle c) {
   {
     const size_t n = (size_t)P.W0 * P.H0;
     const int grid = (int)std::min<size_t>((n + 3) / 4, (size_t)c->num_sms * 64);
+    if (P.patch_store) {
+      pm_patch_kernel<<<grid, 128, c->smem_patch, s>>>(P);
+      ++launches;
+    }
     pm_initial_cost_kernel<<<grid, 128, c->smem_init, s>>>(P);
     ++launches;
   }
@@ -1324,10 +1488,14 @@ int b200pm_run(b200pm_handle c) {
   PM_CUDA(cudaEventElapsedTime(&c->last_ms, c->ev[0], c->ev[2]));
   PM_CUDA(cudaEventElapsedTime(&c->last_sweep_ms, c->ev[1], c->ev[2]));
   c->last_kernel_ms[0] = c->last_kernel_ms[1] = c->last_kernel_ms[2] = 0.0f;
+  c->last_sweep_pass_ms.assign((size_t)t * 3, 0.0f);
   for (int i = 0; i < t; ++i)
     for (int kk = 0; kk < 3; ++kk) {
       float ms = 0.0f;
-      if (cudaEventElapsedTime(&ms, c->sweep_ev[(size_t)i * 4 + kk], c->sweep_ev[(size_t)i * 4 + kk + 1]) == cudaSuccess) c->last_kernel_ms[kk] += ms;
+      if (cudaEventElapsedTime(&ms, c->sweep_ev[(size_t)i * 4 + kk], c->sweep_ev[(size_t)i * 4 + kk + 1]) == cudaSuccess) {
+        c->last_kernel_ms[kk] += ms;
+        c->last_sweep_pass_ms[(size_t)i * 3 + kk] = ms;
+      }
     }
   c->last_launches = launches;
   c->ran = true;
@@ -1338,6 +1506,11 @@ float b200pm_last_run_ms(b200pm_handle c) { return c ? c->last_ms : -1.0f; }
 float b200pm_last_sweep_ms(b200pm_handle c) { return c ? c->last_sweep_ms : -1.0f; }
 int b200pm_last_num_launches(b200pm_handle c) { return c ? c->last_launches : -1; }
 float b200pm_last_pass_ms(b200pm_handle c, int which) { return (c && which >= 0 && which < 3) ? c->last_kernel_ms[which] : -1.0f; }
+float b200pm_last_sweep_pass_ms(b200pm_handle c, int sweep, int which) {
+  if (!c || which < 0 || which >= 3 || sweep < 0 || (size_t)sweep * 3 >= c->last_sweep_pass_ms.size()) return -1.0f;
+  return c->last_sweep_pass_ms[(size_t)sweep * 3 + which];
+}
+size_t b200pm_patch_store_bytes(b200pm_handle c) { return c ? c->patch_store_bytes : 0; }
 
 static int pm_export(b200pm_handle c, float* depth, float* normal, float* sel, uint8_t* mask) {
   if (!c) return pm_fail(-1, "null handle");

@@ -212,6 +212,10 @@ def _bind(lib):
     lib.b200pm_last_num_launches.argtypes = [H]
     lib.b200pm_last_pass_ms.argtypes = [H, ctypes.c_int]
     lib.b200pm_last_pass_ms.restype = ctypes.c_float
+    lib.b200pm_last_sweep_pass_ms.argtypes = [H, ctypes.c_int, ctypes.c_int]
+    lib.b200pm_last_sweep_pass_ms.restype = ctypes.c_float
+    lib.b200pm_patch_store_bytes.argtypes = [H]
+    lib.b200pm_patch_store_bytes.restype = ctypes.c_size_t
     lib.b200pm_get_depth.argtypes = [H, _f32p]
     lib.b200pm_get_normal.argtypes = [H, _f32p]
     lib.b200pm_get_sel_prob.argtypes = [H, _f32p]
@@ -289,6 +293,14 @@ class PatchMatch:
 
     def last_pass_ms(self, which):
         return float(self._lib.b200pm_last_pass_ms(self._h, which))
+
+    def last_sweep_pass_ms(self, sweep, which):
+        """Device time of one pass (0 = rand + msg, 1 = pixel, 2 = serial) in one sweep of the last run."""
+        return float(self._lib.b200pm_last_sweep_pass_ms(self._h, sweep, which))
+
+    def patch_store_bytes(self):
+        """Device bytes of the reference-patch store; 0 when every pass builds the patch inline."""
+        return int(self._lib.b200pm_patch_store_bytes(self._h))
 
     def last_num_launches(self):
         return int(self._lib.b200pm_last_num_launches(self._h))

@@ -106,6 +106,11 @@ int b200pm_last_num_launches(b200pm_handle h);
 /* Device time summed over the sweeps of the last run for one pass of the split sweep: 0 = pm_rand_kernel (column-serial
  * PRNG pass), 1 = pm_pixel_kernel (pixel-parallel NCC pass, the dominant kernel), 2 = pm_serial_kernel. */
 float b200pm_last_pass_ms(b200pm_handle h, int which);
+/* The same for one sweep of the last run (sweep t runs in frame t % 4; -1 for a sweep that did not run). */
+float b200pm_last_sweep_pass_ms(b200pm_handle h, int sweep, int which);
+/* Device bytes of the handle's patch store (every pixel's bilateral reference patch, built once per run); 0 when the
+ * store does not fit its budget (DESIGN.md §2) or B200PM_PATCH_STORE=0, and every pass builds the patch inline. */
+size_t b200pm_patch_store_bytes(b200pm_handle h);
 
 /* PatchMatchCuda::GetDepthMap / GetNormalMap / GetSelProbMap
  * (patch_match_cuda.cu:1354-1365).  Layouts match mvs::Mat<float>: slice-major,
