@@ -142,8 +142,8 @@ __global__ void __launch_bounds__(TT) ba_tile_kernel(const BaTileArgs a) {
 // Diagonal tile k: unblocked Cholesky in shared memory with the pivot test, then the inverse of the factor (one column
 // per thread, forward substitution) into dinv[k].  The factor goes back with a zero upper triangle.
 #define PT 256
-__global__ void __launch_bounds__(PT) ba_tile_potrf_kernel(double* A, int N, int k, int n_check, double pivot_min, double* dinv,
-                                                           BaDenseFlag* flag) {
+__global__ void __launch_bounds__(PT) ba_tile_potrf_kernel(double* A, int N, int k, int n_test0, int n_check, double pivot_min,
+                                                           double* dinv, BaDenseFlag* flag) {
   if (flag->bad) return;
   __shared__ double s[T][T + 1];   // s[c][r]: column-major
   __shared__ int s_bad;
@@ -155,9 +155,10 @@ __global__ void __launch_bounds__(PT) ba_tile_potrf_kernel(double* A, int N, int
   for (int c = 0; c < T; ++c) {
     if (tid == 0) {
       const double d = s[c][c];
-      if (k * T + c < n_check && !(d > pivot_min)) {
+      const int row = k * T + c;
+      if (row < n_check && !(d > (row < n_test0 ? 0.0 : pivot_min))) {
         s_bad = 1;
-        flag->row = k * T + c; flag->pivot = d; __threadfence(); flag->bad = 1;
+        flag->row = row; flag->pivot = d; __threadfence(); flag->bad = 1;
       } else {
         s[c][c] = sqrt(d);
       }
@@ -187,11 +188,12 @@ __global__ void __launch_bounds__(PT) ba_tile_potrf_kernel(double* A, int N, int
   for (int e = tid; e < T * T; e += PT) { const int r = e % T, c = e / T; D[(long long)c * N + r] = r >= c ? s[c][r] : 0.0; }
 }
 
-cudaError_t ba_dense_potrf(double* A, int N, int n_check, double pivot_min, double* dinv, BaDenseFlag* flag, cudaStream_t st) {
+cudaError_t ba_dense_potrf(double* A, int N, int n_test0, int n_check, double pivot_min, double* dinv, BaDenseFlag* flag,
+                           cudaStream_t st) {
   const int nt = N / T;
   BaTileArgs a{A, N, nt, 0, dinv, nullptr, flag};
   for (int k = 0; k < nt; ++k) {
-    ba_tile_potrf_kernel<<<1, PT, 0, st>>>(A, N, k, n_check, pivot_min, dinv, flag);
+    ba_tile_potrf_kernel<<<1, PT, 0, st>>>(A, N, k, n_test0, n_check, pivot_min, dinv, flag);
     const int m = nt - 1 - k;
     if (!m) continue;
     a.step = k;

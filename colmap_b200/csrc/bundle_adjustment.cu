@@ -3517,7 +3517,9 @@ int b200ba_test_pack(const b200ba_options* o, b200ba_problem* p, int64_t capacit
 // never stored in fp32.  S = H_cc - H_cp (H_pp + damping I)^-1 H_pc over the camera-side rows that the reference keeps,
 // ordered [others (sensor_from_rig, intrinsics) | poses], then one dense Cholesky and S^-1 in place (ba_dense_f64.cu).
 // With the others first, the pivots of the pose rows are those of S_cc - S_co S_oo^-1 S_oc, so damping the others'
-// diagonal and factorising once is SchurEliminateOtherParams followed by the reference's rank test on the pose matrix.
+// diagonal and factorising once is SchurEliminateOtherParams followed by the reference's rank test on the pose matrix,
+// provided the rank test starts at the first pose row: the others' rows fail only on a pivot <= 0, as the reference's
+// LLT of S_oo + damping I does (a weakly determined intrinsic is eliminated, not reported).
 // ------------------------------------------------------------------------------------------------
 #define BA_COV_MAX_N 32768
 struct BaCov {
@@ -3714,9 +3716,8 @@ static int ba_cov_impl(const b200ba_options* o, const b200ba_covariance_options*
   }
   if (n > BA_COV_MAX_N)
     return ba_fail(-3, "covariance: reduced matrix dimension " + std::to_string(n) + " above the dense limit " + std::to_string(BA_COV_MAX_N));
-  if (!want_others) {   // the others are eliminated: no blocks of their own (the reference's L_inv has no rows for them)
-    std::fill(H->cam_size.begin(), H->cam_size.end(), 0); std::fill(H->sens_size.begin(), H->sens_size.end(), 0);
-  }
+  // the rank test covers the rows the reference tests: all of S in ALL mode, the poses only when the others are eliminated
+  const int n_test0 = want_others ? 0 : n_others;
   const long long N = (n + BA_TILE - 1) / BA_TILE * BA_TILE;
   BaPool work;            // the solve's device layout and the scratch of this estimate
   BaCovStream G;
@@ -3749,7 +3750,7 @@ static int ba_cov_impl(const b200ba_options* o, const b200ba_covariance_options*
     BaDenseFlag* d_flag; double *dinv, *panel;
     BA_CUDA(work.alloc(&d_flag, 1)); BA_CUDA(work.alloc(&dinv, (size_t)N * BA_TILE)); BA_CUDA(work.alloc(&panel, (size_t)N * BA_TILE));
     BA_CUDA(cudaMemsetAsync(d_flag, 0, sizeof(BaDenseFlag), G.st));
-    BA_CUDA(ba_dense_potrf(C.S, (int)N, n, 1e-6, dinv, d_flag, G.st));
+    BA_CUDA(ba_dense_potrf(C.S, (int)N, n_test0, n, 1e-6, dinv, d_flag, G.st));
     BA_CUDA(cudaEventRecord(G.ev[2], G.st));
     BA_CUDA(ba_dense_potri(C.S, (int)N, dinv, panel, d_flag, G.st));
     BA_CUDA(cudaEventRecord(G.ev[3], G.st));
@@ -3760,8 +3761,12 @@ static int ba_cov_impl(const b200ba_options* o, const b200ba_covariance_options*
   BA_CUDA(cudaStreamSynchronize(G.st));
   if (flag.bad) {
     char b[160];
-    snprintf(b, sizeof(b), "covariance not estimable: pivot %.3g <= 1e-6 at row %d of %d of the reduced matrix (", flag.pivot, flag.row, n);
+    snprintf(b, sizeof(b), "covariance not estimable: pivot %.3g <= %s at row %d of %d of the reduced matrix (", flag.pivot,
+             flag.row < n_test0 ? "0" : "1e-6", flag.row, n);
     return ba_fail(1, std::string(b) + ba_cov_row_name(*H, flag.row) + "): the problem has an unfixed gauge or another degeneracy");
+  }
+  if (!want_others) {   // the others are eliminated: no blocks of their own (the reference's L_inv has no rows for them)
+    std::fill(H->cam_size.begin(), H->cam_size.end(), 0); std::fill(H->sens_size.begin(), H->sens_size.end(), 0);
   }
   for (int k = 0; k < 3; ++k) { float ms = 0; BA_CUDA(cudaEventElapsedTime(&ms, G.ev[k], G.ev[k + 1])); H->ms[1 + k] = ms; }
   H->S = C.S; H->N = N; H->n = n; H->pcov = C.pcov;
@@ -3789,6 +3794,25 @@ static int ba_cov_block(b200ba_covariance* h, int r0, int a, int c0, int b, doub
 }
 
 extern "C" {
+
+// ---- hook for the GPU test tier: the dense kernels alone ----
+// ba_dense_potrf and, when invert != 0, ba_dense_potri on the caller's device matrix A (N x N, column-major, lower
+// triangle, N a multiple of 64), on the legacy default stream.  Returns 0, 1 after a failed pivot (its row and value in
+// bad_row / bad_pivot), or < 0.
+int b200ba_test_dense_f64(double* A, int N, int n_test0, int n_check, double pivot_min, int invert, int* bad_row, double* bad_pivot) {
+  if (!A || !bad_row || !bad_pivot) return ba_fail(-1, "null argument");
+  if (N <= 0 || N % BA_TILE || N > BA_COV_MAX_N) return ba_fail(-2, "N must be a positive multiple of 64 up to 32768");
+  BaPool work;
+  BaDenseFlag flag = {}, *d_flag;
+  double *dinv, *panel;
+  BA_CUDA(work.alloc(&d_flag, 1)); BA_CUDA(work.alloc(&dinv, (size_t)N * BA_TILE)); BA_CUDA(work.alloc(&panel, (size_t)N * BA_TILE));
+  BA_CUDA(cudaMemsetAsync(d_flag, 0, sizeof(BaDenseFlag), 0));
+  BA_CUDA(ba_dense_potrf(A, N, n_test0, n_check, pivot_min, dinv, d_flag, 0));
+  if (invert) BA_CUDA(ba_dense_potri(A, N, dinv, panel, d_flag, 0));
+  BA_CUDA(cudaMemcpy(&flag, d_flag, sizeof(flag), cudaMemcpyDeviceToHost));
+  *bad_row = flag.row; *bad_pivot = flag.pivot;
+  return flag.bad ? 1 : 0;
+}
 
 void b200ba_covariance_options_init(b200ba_covariance_options* c) { c->params = B200BA_COV_ALL; c->damping = 1e-8; }
 

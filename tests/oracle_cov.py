@@ -161,6 +161,34 @@ def _order(columns, kind):
     return [key for key in columns if key[0] == kind]
 
 
+def point_blocks(J, columns, points, damping):
+    """(H_pp + damping I)^-1 per point (H_pp is block diagonal: 3 x 3 per point)."""
+    p_cols = np.concatenate([columns[k] for k in points]) if points else np.zeros(0, np.int64)
+    Jp = J[:, p_cols].tocsc()
+    Hpp = (Jp.T @ Jp).tocoo()
+    blocks = np.zeros((len(points), 3, 3))
+    blocks[Hpp.row // 3, Hpp.row % 3, Hpp.col % 3] = Hpp.data
+    return Jp, (np.linalg.inv(blocks + damping * np.eye(3)) if points else blocks)
+
+
+def reduced_matrix(jac, damping=1e-8):
+    """(S, npose): the Schur complement of the points (with damping) over [poses | others], npose pose rows first."""
+    J, columns = jac
+    poses, points = _order(columns, "pose"), _order(columns, "point")
+    a_keys = poses + _order(columns, "sensor") + _order(columns, "camera")
+    a_cols = np.concatenate([columns[k] for k in a_keys]) if a_keys else np.zeros(0, np.int64)
+    Ja = J[:, a_cols].tocsc()
+    Jp, Hpp_inv = point_blocks(J, columns, points, damping)
+    S = (Ja.T @ Ja).toarray()
+    if points:
+        Hap = (Ja.T @ Jp).tocsr()
+        r = np.arange(3 * len(points)).reshape(-1, 3)
+        Hi = scipy.sparse.csr_matrix((Hpp_inv.reshape(-1), (np.repeat(r, 3, axis=1).reshape(-1), np.tile(r, (1, 3)).reshape(-1))),
+                                     shape=(r.size, r.size))
+        S = S - (Hap @ Hi @ Hap.T).toarray()
+    return S, sum(len(columns[k]) for k in poses)
+
+
 def estimate(options, flat, params=ALL, damping=1e-8, cross=True, jac=None):
     """covariance.cc restated.  Returns (blocks, None) or (None, message) when not estimable.  cross=False: no
     pose-pair blocks; jac: the (J, columns) of jacobian(options, flat), when already formed."""
@@ -170,35 +198,26 @@ def estimate(options, flat, params=ALL, damping=1e-8, cross=True, jac=None):
     want_points, want_poses, want_others = params != POSES, params != POINTS, params == ALL
     out = {}
     a_keys = poses + others
-    a_cols = np.concatenate([columns[k] for k in a_keys]) if a_keys else np.zeros(0, np.int64)
-    p_cols = np.concatenate([columns[k] for k in points]) if points else np.zeros(0, np.int64)
-    Ja, Jp = J[:, a_cols].tocsc(), J[:, p_cols].tocsc()
-    # H_pp is block diagonal (3 x 3 per point): gather the blocks, add the damping, invert them
-    Hpp = (Jp.T @ Jp).tocoo()
-    blocks = np.zeros((len(points), 3, 3))
-    blocks[Hpp.row // 3, Hpp.row % 3, Hpp.col % 3] = Hpp.data
-    Hpp_inv = np.linalg.inv(blocks + damping * np.eye(3)) if points else blocks
     if want_points:
+        Hpp_inv = point_blocks(J, columns, points, damping)[1]
         for n, key in enumerate(points):
             out[key] = Hpp_inv[n]
     if not want_poses:
         return out, None
-    if points:
-        Hap = (Ja.T @ Jp).tocsr()
-        r = np.arange(3 * len(points)).reshape(-1, 3)
-        Hi = scipy.sparse.csr_matrix((Hpp_inv.reshape(-1), (np.repeat(r, 3, axis=1).reshape(-1), np.tile(r, (1, 3)).reshape(-1))),
-                                     shape=(r.size, r.size))
-        S = (Ja.T @ Ja).toarray() - (Hap @ Hi @ Hap.T).toarray()
-    else:
-        S = (Ja.T @ Ja).toarray()
-    npose = sum(len(columns[k]) for k in poses)
+    S, npose = reduced_matrix((J, columns), damping)
     starts, at = {}, 0
     for k in a_keys:
         starts[k] = (at, len(columns[k])); at += len(columns[k])
-    if not want_others:      # SchurEliminateOtherParams
+    if not want_others and npose < len(S):      # SchurEliminateOtherParams: an LLT of S_oo + damping I
         S_cc, S_co, S_oo = S[:npose, :npose], S[:npose, npose:], S[npose:, npose:].copy()
         S_oo[np.diag_indices_from(S_oo)] += damping
-        S = S_cc - S_co @ np.linalg.solve(S_oo, S_co.T) if S_oo.size else S_cc
+        try:
+            Y = scipy.linalg.solve_triangular(np.linalg.cholesky(S_oo), S_co.T, lower=True)
+        except np.linalg.LinAlgError:
+            return None, "others not positive definite"
+        S = S_cc - Y.T @ Y
+    elif not want_others:
+        S = S[:npose, :npose]
     n = S.shape[0]
     if n == 0:
         return out, None

@@ -6,7 +6,8 @@ import pytest
 
 import oracle_ba
 import oracle_cov
-from colmap_b200.bundle_adjustment import (BundleAdjustmentConfig, BundleAdjustmentOptions, GetCovarianceForComposedRigid3d,
+from colmap_b200.bundle_adjustment import (FULL_OPENCV, RAD_TAN_THIN_PRISM_FISHEYE, BundleAdjustmentConfig, BundleAdjustmentOptions,
+                                           GetCovarianceForComposedRigid3d,
                                            GetCovarianceForRelativeRigid3d, GetCovarianceForRigid3dInverse, flatten_reconstruction,
                                            rigid3d_adjoint, rigid3d_adjoint_inverse, rigid3d_inverse)
 from colmap_b200.synthetic import synthesize_ba_problem, synthesize_rig_reconstruction
@@ -74,6 +75,40 @@ def test_masked_pose_sizes():
     est, msg = oracle_cov.estimate(o, flat, oracle_cov.POSES)
     assert est is not None, msg
     assert est[("pose", 1)].shape == (3, 3) and ("camera", 1) not in est
+
+
+def weak_intrinsics_scene(name, solve):
+    """(options, flat): wide-model scenes, solved by `solve`, under a two-cams gauge, whose intrinsics are weakly
+    determined (FULL_OPENCV: k1 against the rational k4) while the poses are not.  The reference eliminates the intrinsics
+    and rank-tests only the reduced pose matrix, so the POSES modes are estimable and ALL is not."""
+    if name == "full_opencv":
+        _, flat = synthesize_ba_problem(12, 600, 6, models=(FULL_OPENCV,), seed=11, point2D_stddev=0.5)
+        options = BundleAdjustmentOptions()
+    else:
+        _, flat = synthesize_ba_problem(16, 1200, 8, models=(RAD_TAN_THIN_PRISM_FISHEYE,), seed=11, point2D_stddev=0.5)
+        options = BundleAdjustmentOptions(refine_principal_point=True)
+    flat.pose_constant = flat.pose_constant.copy(); flat.pose_fixed_dim = flat.pose_fixed_dim.copy()
+    flat.pose_constant[0] = 1
+    flat.pose_fixed_dim[1] = int(np.argmax(np.abs(flat.poses[1, 4:] - flat.poses[0, 4:])))
+    solve(options, flat)
+    return options, flat
+
+
+def test_weak_intrinsics_scene_still_tests_the_rank_test_rows():
+    """Keeps the FULL_OPENCV scene of the GPU POSES-mode tests a case where the rows of the rank test matter: the
+    reference estimates the pose covariances, while a rank test over all rows of S in the [others | poses] order (damping
+    on the others) would stop at an intrinsics pivot <= 1e-6."""
+    options, flat = weak_intrinsics_scene("full_opencv", oracle_ba.solve)
+    jac = oracle_cov.jacobian(options, flat)
+    est, msg = oracle_cov.estimate(options, flat, oracle_cov.POSES, jac=jac)
+    assert est is not None, msg
+    S, npose = oracle_cov.reduced_matrix(jac)
+    order = np.r_[npose:len(S), :npose]
+    S = S[np.ix_(order, order)]
+    no = len(S) - npose
+    S[np.arange(no), np.arange(no)] += 1e-8
+    pivots = np.diag(np.linalg.cholesky(S)) ** 2
+    assert pivots[:no].min() <= 1e-6 and pivots[no:].min() > 1e-6, (pivots[:no].min(), pivots[no:].min())
 
 
 def test_unfixed_gauge_not_estimable():
