@@ -796,11 +796,14 @@ class BundleAdjuster:
             fix_gauge_three_points(flat)
         return flat, image_ids, camera_ids, point_ids
 
+    def _solve_flat(self, flat, pose_ids):
+        return solve_flat(self.options_, flat)
+
     def Solve(self) -> BundleAdjustmentSummary:
         rec = self.reconstruction_
         flat, image_ids, camera_ids, point_ids = self.flat_problem()
         if rec.frames:      # poses are frames, sensors the non-reference cameras
-            summary = solve_flat(self.options_, flat)
+            summary = self._solve_flat(flat, image_ids)
             for k, f in enumerate(image_ids):
                 rec.frames[f].rig_from_world[:] = flat.poses[k]
             for k, c in enumerate(flat.sensor_camera_ids):
@@ -813,7 +816,7 @@ class BundleAdjuster:
             for k, p in enumerate(point_ids):
                 rec.points3D[p].xyz[:] = flat.points[k]
             return summary
-        summary = solve_flat(self.options_, flat)
+        summary = self._solve_flat(flat, image_ids)
         # write back in place (variable blocks only changed)
         for k, i in enumerate(image_ids):
             rec.images[i].cam_from_world[:] = flat.poses[k]
@@ -1042,6 +1045,9 @@ def EstimateBACovariance(options: BACovarianceOptions, reconstruction: Reconstru
     """EstimateBACovariance (covariance.cc): the covariance of the problem `bundle_adjuster` solves, at the parameters
     the reconstruction holds now (call it after Solve()).  None when the problem is not estimable (unfixed gauge)."""
     rec = reconstruction
+    if isinstance(bundle_adjuster, PosePriorBundleAdjuster):
+        raise BundleAdjustmentError("EstimateBACovariance of a pose-prior bundle adjustment is not supported: the covariance "
+                                    "would ignore the prior residuals")
     for image_id in rec.images:
         if not rec.IsRefInFrame(image_id):
             raise BundleAdjustmentError(f"image {image_id} is not the reference sensor of its frame: pose covariances of "
@@ -1061,3 +1067,384 @@ def EstimateBACovariance(options: BACovarianceOptions, reconstruction: Reconstru
             if c in rig.sensors:
                 others.append((rig.sensors[c], "sensor", s))
     return BACovariance(cov, pose_index, {p: k for k, p in enumerate(point_ids)}, others)
+
+
+# ------------------------------------------------------------------------------------------------ pose priors
+# PosePriorBundleAdjuster (bundle_adjustment_ceres.cc:900-1080) over include/b200_ba_pose_prior.h.  The alignment to the
+# priors and the normalisation happen here on the host, as the reference does them before it builds the problem; the GPU
+# solve receives the priors already in the normalized frame.
+CHI_SQUARE_95_THREE_DOF = 7.814727903251179
+
+
+class _CPositionPriors(ctypes.Structure):
+    _fields_ = [("num_priors", ctypes.c_int), ("pose_idx", _i32p), ("sensor_idx", _i32p), ("position", _f64p),
+                ("covariance", _f64p), ("loss_function_type", ctypes.c_int), ("loss_function_scale", ctypes.c_double)]
+
+
+class FlatPositionPriors:
+    """Arrays behind a b200ba_position_priors (kept alive here).  pose_idx / sensor_idx index the FlatProblem."""
+
+    def __init__(self, pose_idx, sensor_idx, position, covariance, loss_function_type=TRIVIAL,
+                 loss_function_scale=float(np.sqrt(CHI_SQUARE_95_THREE_DOF))):
+        c = np.ascontiguousarray
+        self.pose_idx = c(pose_idx, np.int32).reshape(-1)
+        self.sensor_idx = c(sensor_idx, np.int32).reshape(-1)
+        self.position = c(position, np.float64).reshape(-1, 3)
+        self.covariance = c(covariance, np.float64).reshape(-1, 3, 3)
+        self.loss_function_type, self.loss_function_scale = int(loss_function_type), float(loss_function_scale)
+
+    def __len__(self):
+        return len(self.pose_idx)
+
+    def to_c(self) -> _CPositionPriors:
+        n = len(self.pose_idx)
+        if not (len(self.sensor_idx) == len(self.position) == len(self.covariance) == n):
+            raise ValueError("prior arrays differ in length")
+        return _CPositionPriors(n, self.pose_idx.ctypes.data_as(_i32p), self.sensor_idx.ctypes.data_as(_i32p),
+                                self.position.ctypes.data_as(_f64p), self.covariance.ctypes.data_as(_f64p),
+                                self.loss_function_type, self.loss_function_scale)
+
+
+def _bind_prior(lib):
+    if getattr(lib, "_prior_bound", False):
+        return lib
+    _bind(lib)
+    lib.b200ba_solve_with_position_priors.argtypes = [ctypes.POINTER(_COptions), ctypes.POINTER(_CProblem),
+                                                      ctypes.POINTER(_CPositionPriors), ctypes.POINTER(_CSummary)]
+    lib.b200ba_position_priors_init.argtypes = [ctypes.POINTER(_CPositionPriors)]
+    lib.b200ba_position_priors_init.restype = None
+    lib.b200ba_test_prior_position.argtypes = [_f64p, _f64p, _f64p, _f64p, _f64p, _f64p]
+    lib.b200ba_test_prior_position.restype = None
+    lib.b200ba_test_prior_weight.argtypes = [_f64p, _f64p]
+    lib._prior_bound = True
+    return lib
+
+
+def solve_flat_with_position_priors(options: BundleAdjustmentOptions, flat: FlatProblem,
+                                    priors: FlatPositionPriors) -> BundleAdjustmentSummary:
+    """b200ba_solve_with_position_priors; flat is updated in place like solve_flat."""
+    lib = _bind_prior(load_library())
+    co, cp, cpr, cs = options.to_c(), flat.to_c(), priors.to_c(), _CSummary()
+    rc = lib.b200ba_solve_with_position_priors(ctypes.byref(co), ctypes.byref(cp), ctypes.byref(cpr), ctypes.byref(cs))
+    if rc != 0:
+        raise BundleAdjustmentError(f"b200ba_solve_with_position_priors failed ({rc}): {lib.b200ba_last_error().decode()}")
+    return BundleAdjustmentSummary.from_c(cs)
+
+
+@dataclass
+class PosePrior:
+    """PosePrior (geometry/pose_prior.h) for a CAMERA sensor: a Cartesian position of the image's projection centre; a NaN
+    covariance means none was given."""
+    image_id: int
+    position: np.ndarray = field(default_factory=lambda: np.full(3, np.nan))
+    position_covariance: np.ndarray = field(default_factory=lambda: np.full((3, 3), np.nan))
+    sensor_type: str = "CAMERA"
+
+    def HasPosition(self) -> bool:
+        return bool(np.all(np.isfinite(self.position)))
+
+    def HasPositionCov(self) -> bool:
+        return bool(np.all(np.isfinite(self.position_covariance)))
+
+
+@dataclass
+class RANSACOptions:
+    """RANSACOptions (optim/ransac.h:50-90); max_error <= 0 lets AlignReconstructionToPosePriors choose it."""
+    max_error: float = 0.0
+    min_inlier_ratio: float = 0.1
+    confidence: float = 0.99
+    dyn_num_trials_multiplier: float = 3.0
+    min_num_trials: int = 0
+    max_num_trials: int = 100000
+    random_seed: int = -1
+
+
+@dataclass
+class PosePriorBundleAdjustmentOptions:
+    """PosePriorBundleAdjustmentOptions (bundle_adjustment.h:236-270) with the Ceres prior-loss options
+    (bundle_adjustment_ceres.h:102-112)."""
+    prior_position_fallback_stddev: float = 1.0
+    alignment_ransac_options: RANSACOptions = field(default_factory=RANSACOptions)
+    prior_position_loss_function_type: int = TRIVIAL
+    prior_position_loss_scale: float = float(np.sqrt(CHI_SQUARE_95_THREE_DOF))
+
+    def Check(self) -> bool:
+        return self.prior_position_fallback_stddev > 0 and self.prior_position_loss_scale > 0
+
+
+class Sim3d:
+    """Sim3d (geometry/sim3.h): x_new = scale * R(q) x + t, q = (x, y, z, w)."""
+
+    def __init__(self, scale=1.0, rotation=(0.0, 0.0, 0.0, 1.0), translation=(0.0, 0.0, 0.0)):
+        self.scale = float(scale)
+        self.rotation = np.asarray(rotation, np.float64)
+        self.translation = np.asarray(translation, np.float64)
+
+    def R(self):
+        return _quat_to_R(self.rotation)
+
+    def __mul__(self, x):
+        return self.scale * (np.asarray(x, np.float64) @ self.R().T) + self.translation
+
+    def inverse(self) -> "Sim3d":
+        qi = np.array([-self.rotation[0], -self.rotation[1], -self.rotation[2], self.rotation[3]])
+        return Sim3d(1.0 / self.scale, qi, -(_quat_to_R(qi) @ self.translation) / self.scale)
+
+
+def _R_to_quat(R):
+    """Eigen::Quaterniond(Matrix3d), (x, y, z, w)"""
+    t = np.trace(R)
+    if t > 0:
+        s = np.sqrt(t + 1.0) * 2
+        q = np.array([(R[2, 1] - R[1, 2]) / s, (R[0, 2] - R[2, 0]) / s, (R[1, 0] - R[0, 1]) / s, 0.25 * s])
+    else:
+        i = int(np.argmax(np.diag(R)))
+        j, k = (i + 1) % 3, (i + 2) % 3
+        s = np.sqrt(R[i, i] - R[j, j] - R[k, k] + 1.0) * 2
+        q = np.zeros(4)
+        q[i] = 0.25 * s
+        q[j] = (R[j, i] + R[i, j]) / s
+        q[k] = (R[k, i] + R[i, k]) / s
+        q[3] = (R[k, j] - R[j, k]) / s
+    return q / np.linalg.norm(q)
+
+
+def estimate_sim3_umeyama(src, tgt) -> Optional[Sim3d]:
+    """Umeyama's least-squares similarity tgt ~ s R src + t (Eigen::umeyama, as SimilarityTransformEstimator uses it)."""
+    src, tgt = np.asarray(src, np.float64), np.asarray(tgt, np.float64)
+    n = len(src)
+    if n < 3:
+        return None
+    ms, mt = src.mean(0), tgt.mean(0)
+    xs, xt = src - ms, tgt - mt
+    C = xt.T @ xs / n
+    U, d, Vt = np.linalg.svd(C)
+    S = np.ones(3)
+    if np.linalg.det(U) * np.linalg.det(Vt) < 0:
+        S[2] = -1
+    R = U @ np.diag(S) @ Vt
+    var_s = (xs ** 2).sum() / n
+    if not var_s > 0:
+        return None
+    scale = float((d * S).sum() / var_s)
+    if not (np.isfinite(scale) and scale > 0):
+        return None
+    return Sim3d(scale, _R_to_quat(R), mt - scale * (R @ ms))
+
+
+def estimate_sim3_robust(src, tgt, ransac: RANSACOptions):
+    """EstimateSim3dRobust: LO-RANSAC over Umeyama's minimal (3-point) fits with a local refit on the inliers; the inlier
+    test is the squared error against max_error^2.  Seeded by ransac.random_seed (-1: a fixed default seed, so the result
+    is reproducible).  Returns (Sim3d or None, inlier mask)."""
+    src, tgt = np.asarray(src, np.float64), np.asarray(tgt, np.float64)
+    n = len(src)
+    if n < 3 or not ransac.max_error > 0:
+        return None, np.zeros(n, bool)
+    rng = np.random.default_rng(ransac.random_seed if ransac.random_seed >= 0 else 0)
+    thr2 = ransac.max_error ** 2
+
+    def inliers_of(T):
+        return ((tgt - T * src) ** 2).sum(1) <= thr2
+
+    best, best_mask, best_n = None, np.zeros(n, bool), 0
+    max_trials, trial = ransac.max_num_trials, 0
+    while trial < max_trials:
+        trial += 1
+        idx = rng.choice(n, 3, replace=False)
+        T = estimate_sim3_umeyama(src[idx], tgt[idx])
+        if T is None:
+            continue
+        mask = inliers_of(T)
+        if mask.sum() > best_n:
+            for _ in range(10):      # local optimisation: refit on the inliers while their number grows
+                T2 = estimate_sim3_umeyama(src[mask], tgt[mask])
+                if T2 is None:
+                    break
+                m2 = inliers_of(T2)
+                if m2.sum() < mask.sum():
+                    break
+                T, grew, mask = T2, m2.sum() > mask.sum(), m2
+                if not grew:
+                    break
+            best, best_mask, best_n = T, mask, int(mask.sum())
+            ratio = best_n / n
+            # dynamic trial count (RANSAC::ComputeNumTrials)
+            nom = 1.0 - ransac.confidence
+            denom = 1.0 - ratio ** 3
+            needed = 0 if denom <= 0 else int(np.ceil(np.log(nom) / np.log(denom) * ransac.dyn_num_trials_multiplier)) if nom > 0 else max_trials
+            max_trials = min(ransac.max_num_trials, max(ransac.min_num_trials, needed))
+    if best is None or best_n < 3 or best_n / n < ransac.min_inlier_ratio:
+        return None, best_mask
+    return best, best_mask
+
+
+def align_reconstruction_to_pose_priors(rec: Reconstruction, pose_priors, ransac: RANSACOptions,
+                                        fallback_stddev: float) -> Optional[Sim3d]:
+    """AlignReconstructionToPosePriors (alignment.cc:240-299): robust Sim3 from projection centres to prior positions.
+    None when fewer than three priors apply or the fit fails."""
+    if not fallback_stddev > 0:
+        raise ValueError("prior_position_fallback_stddev must be positive")
+    by_image = {}
+    for pp in pose_priors:
+        if pp.sensor_type == "CAMERA" and pp.HasPosition():
+            if pp.image_id in by_image:
+                raise ValueError(f"duplicate pose prior for image {pp.image_id}")
+            by_image[pp.image_id] = pp
+    src, tgt, rms_vars = [], [], []
+    for image_id in sorted(rec.images):
+        pp = by_image.get(image_id)
+        if pp is None:
+            continue
+        src.append(projection_center(rec, image_id))
+        tgt.append(pp.position)
+        tr = float(np.trace(pp.position_covariance))
+        if tr > 0.0:
+            rms_vars.append(tr / 3.0)
+    if len(src) < 3:
+        return None
+    ransac = RANSACOptions(**vars(ransac))
+    if ransac.max_error <= 0:
+        ransac.max_error = automatic_alignment_max_error(rms_vars, fallback_stddev)
+    T, _ = estimate_sim3_robust(np.array(src), np.array(tgt), ransac)
+    return T
+
+
+def automatic_alignment_max_error(rms_vars, fallback_stddev):
+    """sqrt(chi2_95(3) * median(trace(cov) / 3)); the fallback variance when no prior has a covariance.  The median of an
+    even count is the mean of the two middle values (colmap Median)."""
+    v = list(rms_vars) if len(rms_vars) else [fallback_stddev * fallback_stddev]
+    return float(np.sqrt(CHI_SQUARE_95_THREE_DOF * np.median(v)))
+
+
+def _image_cam_from_world(rec: Reconstruction, image_id):
+    im = rec.images[image_id]
+    if im.frame_id is None:
+        return im.cam_from_world
+    fr = rec.frames[im.frame_id]
+    rig = rec.rigs[fr.rig_id]
+    if rig.ref_sensor == im.camera_id:
+        return fr.rig_from_world
+    return _rigid_compose(rig.sensors[im.camera_id], fr.rig_from_world)
+
+
+def projection_center(rec: Reconstruction, image_id):
+    """Image::ProjectionCenter: -R^T t of cam_from_world."""
+    T = _image_cam_from_world(rec, image_id)
+    return -_quat_to_R(T[:4]).T @ T[4:]
+
+
+def _transform_camera_world(sim: Sim3d, cam_from_world):
+    """TransformCameraWorld (geometry/sim3.cc): the same camera in the new world, its translation scaled."""
+    R = _quat_to_R(cam_from_world[:4]) @ sim.R().T
+    t = sim.scale * cam_from_world[4:] - R @ sim.translation
+    return np.concatenate([_R_to_quat(R), t])
+
+
+def transform_reconstruction(rec: Reconstruction, new_from_old: Sim3d):
+    """Reconstruction::Transform (reconstruction.cc:788-805): sensor_from_rig translations scaled, rig_from_world (or the
+    image pose of a trivial frame) and the points moved to the new world."""
+    for rig in rec.rigs.values():
+        for T in rig.sensors.values():
+            T[4:] *= new_from_old.scale
+    if rec.frames:
+        for fr in rec.frames.values():
+            fr.rig_from_world[:] = _transform_camera_world(new_from_old, fr.rig_from_world)
+    else:
+        for im in rec.images.values():
+            im.cam_from_world[:] = _transform_camera_world(new_from_old, im.cam_from_world)
+    for pt in rec.points3D.values():
+        pt.xyz[:] = new_from_old * pt.xyz
+
+
+def normalization_centroid(centers, min_percentile=0.1, max_percentile=0.9):
+    """ComputeBoundingBoxAndCentroid (geometry/normalization.cc:39-90): per axis, the mean of the order statistics
+    floor(min_p * (n - 1)) .. ceil(max_p * (n - 1))."""
+    c = np.sort(np.asarray(centers, np.float64), axis=0)
+    end = len(c) - 1
+    lo, hi = min(end, int(np.floor(min_percentile * end))), min(end, int(np.ceil(max_percentile * end)))
+    return c[lo:hi + 1].mean(0)
+
+
+def normalize_reconstruction(rec: Reconstruction, fixed_scale=True, extent=10.0, min_percentile=0.1, max_percentile=0.9) -> Sim3d:
+    """Reconstruction::Normalize(fixed_scale, extent, percentiles, use_images=true) (reconstruction.cc:698-728)."""
+    centers = [projection_center(rec, i) for i in sorted(rec.images)]
+    nreg = len(rec.frames) if rec.frames else len(rec.images)
+    if nreg < 2:
+        return Sim3d()
+    centroid = normalization_centroid(centers, min_percentile, max_percentile)
+    scale = 1.0
+    if not fixed_scale:
+        c = np.sort(np.asarray(centers), axis=0)
+        end = len(c) - 1
+        lo, hi = min(end, int(np.floor(min_percentile * end))), min(end, int(np.ceil(max_percentile * end)))
+        old_extent = float(np.linalg.norm(c[hi] - c[lo]))
+        if old_extent >= np.finfo(float).eps:
+            scale = extent / old_extent
+    tform = Sim3d(scale, (0.0, 0.0, 0.0, 1.0), -scale * centroid)
+    transform_reconstruction(rec, tform)
+    return tform
+
+
+def filter_pose_priors(pose_priors, config: BundleAdjustmentConfig):
+    """The constructor's filter (bundle_adjustment_ceres.cc:915-925): a position, a CAMERA sensor, an image in the config."""
+    return [pp for pp in pose_priors if pp.HasPosition() and pp.sensor_type == "CAMERA" and config.HasImage(pp.image_id)]
+
+
+class PosePriorBundleAdjuster(BundleAdjuster):
+    """PosePriorBundleAdjuster (bundle_adjustment_ceres.cc:900-1080), B200 backend.  The constructor filters the priors,
+    aligns the reconstruction to them and normalises it (or, with fewer than three priors or a failed alignment, fixes
+    the TWO_CAMS_FROM_WORLD gauge), so Config().FixedGauge() is final before Solve()."""
+
+    def __init__(self, options, prior_options: PosePriorBundleAdjustmentOptions, config, pose_priors, reconstruction):
+        if not prior_options.Check():
+            raise ValueError("invalid PosePriorBundleAdjustmentOptions")
+        super().__init__(options, config, reconstruction)
+        self.prior_options_ = prior_options
+        self.pose_priors_ = filter_pose_priors(pose_priors, config)
+        self.normalized_from_metric_ = Sim3d()
+        self.use_prior_position_ = False
+        if len(self.pose_priors_) >= 3:
+            metric_from_orig = align_reconstruction_to_pose_priors(
+                reconstruction, self.pose_priors_, prior_options.alignment_ransac_options,
+                prior_options.prior_position_fallback_stddev)
+            if metric_from_orig is not None:
+                transform_reconstruction(reconstruction, metric_from_orig)
+                self.use_prior_position_ = True
+        if self.use_prior_position_:
+            self.normalized_from_metric_ = normalize_reconstruction(reconstruction, fixed_scale=True)
+        else:
+            config.FixGauge(TWO_CAMS_FROM_WORLD)
+
+    def flat_priors(self, flat: FlatProblem, pose_ids) -> FlatPositionPriors:
+        """The priors of the parameterized images, in the normalized frame, indexed into `flat` (AddImagePosePriorToProblem,
+        bundle_adjustment_ceres.cc:987-1039; the library skips those whose blocks are all constant)."""
+        rec, po = self.reconstruction_, self.prior_options_
+        pose_index = {p: k for k, p in enumerate(pose_ids)}
+        sensor_of_cam = {c: k for k, c in enumerate(getattr(flat, "sensor_camera_ids", []))}
+        sR = self.normalized_from_metric_.scale * self.normalized_from_metric_.R()
+        pose_idx, sensor_idx, pos, cov = [], [], [], []
+        if self.use_prior_position_:
+            for pp in self.pose_priors_:
+                if pp.image_id not in flat.parameterized_image_ids:
+                    continue
+                im = rec.images[pp.image_id]
+                pose_idx.append(pose_index[im.frame_id if rec.frames else pp.image_id])
+                sensor_idx.append(-1 if rec.IsRefInFrame(pp.image_id) else sensor_of_cam[im.camera_id])
+                pos.append(self.normalized_from_metric_ * pp.position)
+                C = pp.position_covariance if pp.HasPositionCov() else po.prior_position_fallback_stddev ** 2 * np.eye(3)
+                cov.append(sR @ C @ sR.T)
+        return FlatPositionPriors(pose_idx, sensor_idx, np.reshape(pos, (-1, 3)), np.reshape(cov, (-1, 3, 3)),
+                                  po.prior_position_loss_function_type, po.prior_position_loss_scale)
+
+    def _solve_flat(self, flat, pose_ids):
+        return solve_flat_with_position_priors(self.options_, flat, self.flat_priors(flat, pose_ids))
+
+    def Solve(self) -> BundleAdjustmentSummary:
+        summary = super().Solve()
+        transform_reconstruction(self.reconstruction_, self.normalized_from_metric_.inverse())
+        return summary
+
+
+def CreatePosePriorBundleAdjuster(options, prior_options, config, pose_priors, reconstruction) -> PosePriorBundleAdjuster:
+    """Factory (bundle_adjustment.cc:373-390); this build has exactly one backend."""
+    return PosePriorBundleAdjuster(options, prior_options, config, pose_priors, reconstruction)

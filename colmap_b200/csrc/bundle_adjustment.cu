@@ -30,6 +30,7 @@
 
 #include "../../include/b200_bundle_adjustment.h"
 #include "../../include/b200_ba_covariance.h"
+#include "../../include/b200_ba_pose_prior.h"
 #include "device_cache.h"
 #include "ba_models.cuh"
 #include "ba_dense_f64.h"
@@ -290,6 +291,17 @@ struct BaDev {
   double *x, *rr, *z, *p, *q, *dp;
   double* Sd;   // dense reduced camera matrix [nc*nc] (DENSE_SCHUR path), column-major == row-major (symmetric)
   BaCtl* ctl;
+};
+
+struct BaPrior {          // position priors of one solve (n = 0: none, and no prior launch happens; see ba_prior_position)
+  int n = 0, loss_type = 0;
+  double loss_scale = 1.0;
+  const int4* idx = nullptr;   // {pose index, sensor index or -1, pose offset or -1, offset of the sensor tangent or -1}
+  const double* c = nullptr;   // [3n] prior positions
+  const double* W = nullptr;   // [9n] chol(cov^-1)^T, row-major
+  double* J = nullptr;         // [36n] rows of the weighted, loss-corrected (scaled after iteration 0) Jacobian: 3 x [pose 6 | sensor 6]
+  double* r = nullptr;         // [3n] loss-corrected weighted residual
+  double* cost = nullptr;      // [n] 1/2 rho at the linearisation point
 };
 
 __device__ __forceinline__ double ba_block_sum(double v, double* sm) {
@@ -2102,11 +2114,13 @@ static void ba_launch_spmv(const BaDev& D, const BaPath& P, cudaStream_t s) {
     ba_cam_stream_loop_kernel<DC><<<grid, BA_BLOCK, 0, s>>>(D, D.q, 1, tpw);
   }
 }
+__global__ void ba_prior_dense_kernel(const BaDev D, const BaPrior P);
 template <int DC>
-static void ba_launch_dense(const BaDev& D, cudaStream_t s) {
+static void ba_launch_dense(const BaDev& D, const BaPrior& P, cudaStream_t s) {
   cudaMemsetAsync(D.Sd, 0, sizeof(double) * (size_t)D.nc * D.nc, s);
   ba_dense_gram_kernel<DC><<<D.nblocks, BA_BLOCK, 0, s>>>(D);
   if (D.nvpt) ba_dense_schur_kernel<DC><<<(D.nvpt + BA_BLOCK / 32 - 1) / (BA_BLOCK / 32), BA_BLOCK, 0, s>>>(D);
+  if (P.n) ba_prior_dense_kernel<<<(P.n + 255) / 256, 256, 0, s>>>(D, P);
   ba_dense_solve_kernel<<<1, BA_DENSE_T, 0, s>>>(D);
 }
 template <int DC>
@@ -2377,7 +2391,8 @@ struct BaReducer {
   }
 };
 
-static int ba_solve_impl(const b200ba_options* o, b200ba_problem* p, b200ba_summary* sum, b200ba_comm* comm);
+static int ba_solve_impl(const b200ba_options* o, b200ba_problem* p, b200ba_summary* sum, b200ba_comm* comm,
+                         const b200ba_position_priors* priors = nullptr);
 
 extern "C" {
 
@@ -3120,6 +3135,268 @@ static int ba_upload(const BaLayout& L, const b200ba_options* o, const b200ba_pr
   BA_CUDA(cudaStreamSynchronize(st));
   return 0;
 }
+// ---- position priors (PosePriorBundleAdjuster, bundle_adjustment_ceres.cc:987-1039; DESIGN.md §3) ----
+// One covariance-weighted 3-vector residual per prior on camera-side blocks only (a frame's rig_from_world and, for a
+// non-reference sensor, its sensor_from_rig), so the priors add to the reduced camera matrix directly and never enter the
+// point elimination.  Everything per prior is fp64 and one thread per prior; each LM phase gets one extra launch, and
+// only when the solve has priors.
+// AbsolutePosePositionPriorCostFunctor / AbsoluteRigPosePositionPriorCostFunctor (cost_functions/pose_prior.h:75-126):
+// r = c + R^T t of cam_from_world = sensor_from_rig * rig_from_world (sensor == nullptr: identity), and its Jacobians in the
+// tangent space of ba_quat_plus, [rotation | translation], 3x6 row-major.  Plus multiplies by [sin|d| d/|d|, cos|d|] on
+// the left, i.e. R' = (I + 2 [d]x) R to first order, so d(R^T u)/dd = 2 R^T [u]x.
+BA_HD void ba_prior_position(const double* rig, const double* sensor, const double* c, double* res, double* Jr, double* Js) {
+  double Rr[9], Rs[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}, ts[3] = {0, 0, 0};
+  ba_quat_to_R(rig, Rr);
+  if (sensor) { ba_quat_to_R(sensor, Rs); ts[0] = sensor[4]; ts[1] = sensor[5]; ts[2] = sensor[6]; }
+  double v[3], u[3];   // v = R_s^T t_s, u = v + t_r
+  for (int a = 0; a < 3; ++a) { v[a] = Rs[a] * ts[0] + Rs[3 + a] * ts[1] + Rs[6 + a] * ts[2]; u[a] = v[a] + rig[4 + a]; }
+  double A[9];         // A = R_r^T R_s^T
+  for (int a = 0; a < 3; ++a)
+    for (int b = 0; b < 3; ++b) A[3 * a + b] = Rr[a] * Rs[3 * b] + Rr[3 + a] * Rs[3 * b + 1] + Rr[6 + a] * Rs[3 * b + 2];
+  for (int a = 0; a < 3; ++a) res[a] = c[a] + Rr[a] * u[0] + Rr[3 + a] * u[1] + Rr[6 + a] * u[2];
+  const double ux[9] = {0, -u[2], u[1], u[2], 0, -u[0], -u[1], u[0], 0};
+  const double tx[9] = {0, -ts[2], ts[1], ts[2], 0, -ts[0], -ts[1], ts[0], 0};
+  for (int a = 0; a < 3; ++a)
+    for (int j = 0; j < 3; ++j) {
+      Jr[6 * a + j] = 2.0 * (Rr[a] * ux[j] + Rr[3 + a] * ux[3 + j] + Rr[6 + a] * ux[6 + j]);
+      Jr[6 * a + 3 + j] = Rr[3 * j + a];
+      Js[6 * a + j] = sensor ? 2.0 * (A[3 * a] * tx[j] + A[3 * a + 1] * tx[3 + j] + A[3 * a + 2] * tx[6 + j]) : 0.0;
+      Js[6 * a + 3 + j] = sensor ? A[3 * a + j] : 0.0;
+    }
+}
+// weight chol(cov^-1)^T (CovarianceWeightedCostFunctor::LeftSqrtInformation) of a symmetric positive definite 3x3
+// covariance; false when it is not finite, not symmetric or not positive definite
+static bool ba_prior_weight(const double* C, double* W) {
+  double scale = 0.0;
+  for (int k = 0; k < 9; ++k) { if (!std::isfinite(C[k])) return false; scale = std::max(scale, fabs(C[k])); }
+  for (int a = 0; a < 3; ++a)
+    for (int b = 0; b < a; ++b) if (fabs(C[3 * a + b] - C[3 * b + a]) > 1e-12 * scale) return false;
+  // positive definite: the leading minors
+  const double m1 = C[0], m2 = C[0] * C[4] - C[1] * C[3];
+  const double c00 = C[4] * C[8] - C[5] * C[7], c01 = C[5] * C[6] - C[3] * C[8], c02 = C[3] * C[7] - C[4] * C[6];
+  const double det = C[0] * c00 + C[1] * c01 + C[2] * c02;
+  if (!(m1 > 0.0) || !(m2 > 0.0) || !(det > 0.0)) return false;
+  const double id = 1.0 / det;
+  const double I[9] = {c00 * id, (C[2] * C[7] - C[1] * C[8]) * id, (C[1] * C[5] - C[2] * C[4]) * id,
+                       c01 * id, (C[0] * C[8] - C[2] * C[6]) * id, (C[2] * C[3] - C[0] * C[5]) * id,
+                       c02 * id, (C[1] * C[6] - C[0] * C[7]) * id, (C[0] * C[4] - C[1] * C[3]) * id};
+  double L[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};   // lower Cholesky factor of the information matrix (its lower triangle)
+  for (int j = 0; j < 3; ++j) {
+    double d = I[4 * j];
+    for (int k = 0; k < j; ++k) d -= L[3 * j + k] * L[3 * j + k];
+    if (!(d > 0.0)) return false;
+    L[4 * j] = sqrt(d);
+    for (int r = j + 1; r < 3; ++r) {
+      double t = I[3 * r + j];
+      for (int k = 0; k < j; ++k) t -= L[3 * r + k] * L[3 * j + k];
+      L[3 * r + j] = t / L[4 * j];
+    }
+  }
+  for (int a = 0; a < 3; ++a) for (int b = 0; b < 3; ++b) W[3 * a + b] = L[3 * b + a];
+  return std::isfinite(W[0]) && std::isfinite(W[4]) && std::isfinite(W[8]);
+}
+// weighted residual (and, when Jw is set, its weighted tangent Jacobian 3 x 12 [pose | sensor] with the columns of constant
+// blocks and of masked pose dimensions zero) of prior k at (poses, sensors)
+__device__ __forceinline__ void ba_prior_eval(const BaDev& D, const BaPrior& P, int k, const double* poses, const double* sensors,
+                                              double* rw, double* Jw) {
+  const int4 ix = P.idx[k];
+  double pose[7], sens[7], c[3], res[3], Jr[18], Js[18];
+  for (int j = 0; j < 7; ++j) pose[j] = poses[7 * (long long)ix.x + j];
+  if (ix.y >= 0) for (int j = 0; j < 7; ++j) sens[j] = sensors[7 * (long long)ix.y + j];
+  for (int j = 0; j < 3; ++j) c[j] = P.c[3 * (long long)k + j];
+  ba_prior_position(pose, ix.y >= 0 ? sens : nullptr, c, res, Jr, Js);
+  const double* W = P.W + 9 * (long long)k;
+  for (int a = 0; a < 3; ++a) rw[a] = W[3 * a] * res[0] + W[3 * a + 1] * res[1] + W[3 * a + 2] * res[2];
+  if (!Jw) return;
+  const unsigned m = ix.z >= 0 ? D.pose_mask[ix.x] : 0u;
+  for (int a = 0; a < 3; ++a)
+    for (int j = 0; j < 6; ++j) {
+      const double jr = W[3 * a] * Jr[j] + W[3 * a + 1] * Jr[6 + j] + W[3 * a + 2] * Jr[12 + j];
+      const double js = W[3 * a] * Js[j] + W[3 * a + 1] * Js[6 + j] + W[3 * a + 2] * Js[12 + j];
+      Jw[12 * a + j] = ((m >> j) & 1u) ? jr : 0.0;
+      Jw[12 * a + 6 + j] = ix.w >= 0 ? js : 0.0;
+    }
+}
+// camera-side offset of column j of a prior's Jacobian, or -1
+__device__ __forceinline__ int ba_prior_col(const int4& ix, int j) { return j < 6 ? (ix.z >= 0 ? ix.z + j : -1) : (ix.w >= 0 ? ix.w + j - 6 : -1); }
+// linearisation: residual, Jacobian (ceres Corrector with the priors' loss, Jacobi scaling when apply_scale), cost
+__global__ void __launch_bounds__(BA_BLOCK) ba_prior_linearize_kernel(const BaDev D, const BaPrior P, int apply_scale) {
+  __shared__ double sm[8];
+  const int k = blockIdx.x * BA_BLOCK + threadIdx.x;
+  double cost = 0.0;
+  if (k < P.n) {
+    double rw[3], J[36], rho[3];
+    ba_prior_eval(D, P, k, D.poses, D.sensors, rw, J);
+    const double sq = rw[0] * rw[0] + rw[1] * rw[1] + rw[2] * rw[2];
+    ba_loss(P.loss_type, P.loss_scale, sq, rho);
+    cost = 0.5 * rho[0];
+    double rs = 1.0;
+    if (P.loss_type != B200BA_LOSS_TRIVIAL) {
+      const double sqrt_rho1 = sqrt(rho[1]);
+      double alpha_sq_norm = 0.0;
+      rs = sqrt_rho1;
+      if (sq != 0.0 && rho[2] > 0.0) {
+        const double alpha = 1.0 - sqrt(1.0 + 2.0 * sq * rho[2] / rho[1]);
+        rs = sqrt_rho1 / (1 - alpha);
+        alpha_sq_norm = alpha / sq;
+      }
+      for (int j = 0; j < 12; ++j) {
+        const double rj = rw[0] * J[j] + rw[1] * J[12 + j] + rw[2] * J[24 + j];
+        for (int a = 0; a < 3; ++a) J[12 * a + j] = sqrt_rho1 * (J[12 * a + j] - alpha_sq_norm * rw[a] * rj);
+      }
+    }
+    const int4 ix = P.idx[k];
+    for (int j = 0; j < 12; ++j) {
+      const int col = ba_prior_col(ix, j);
+      const double sc = (apply_scale && col >= 0) ? D.scale_c[col] : 1.0;
+      for (int a = 0; a < 3; ++a) P.J[36 * (long long)k + 12 * a + j] = J[12 * a + j] * sc;
+    }
+    for (int a = 0; a < 3; ++a) P.r[3 * (long long)k + a] = rs * rw[a];
+    P.cost[k] = cost;
+  }
+  const double t = ba_block_sum(cost, sm);
+  if (threadIdx.x == 0) atomicAdd(&D.ctl->cost, t);
+}
+// iteration 0: squared column norms of the unscaled prior rows into scale_c (before ba_make_scale_kernel)
+__global__ void ba_prior_colnorm_kernel(const BaDev D, const BaPrior P) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= P.n) return;
+  const int4 ix = P.idx[k];
+  const double* J = P.J + 36 * (long long)k;
+  for (int j = 0; j < 12; ++j) {
+    const int col = ba_prior_col(ix, j);
+    if (col >= 0) atomicAdd(&D.scale_c[col], J[j] * J[j] + J[12 + j] * J[12 + j] + J[24 + j] * J[24 + j]);
+  }
+}
+// build: J^T J into the diagonal blocks H_bb (the pose block; the sensor part of the camera block) and J^T r into g_c
+__global__ void ba_prior_build_kernel(const BaDev D, const BaPrior P) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= P.n) return;
+  const int4 ix = P.idx[k];
+  const double* J = P.J + 36 * (long long)k;
+  const double* r = P.r + 3 * (long long)k;
+  for (int blk = 0; blk < 2; ++blk) {
+    const int off = blk == 0 ? ix.z : ix.w, j0 = 6 * blk;
+    if (off < 0) continue;
+    const int b = D.off2blk[off], n = D.blk_start[b + 1] - D.blk_start[b], l0 = off - D.blk_start[b];
+    double* H = D.Hbb + D.blk_pack[b];
+    for (int i = 0; i < 6; ++i) {
+      atomicAdd(&D.gc[off + i], J[j0 + i] * r[0] + J[12 + j0 + i] * r[1] + J[24 + j0 + i] * r[2]);
+      for (int j = 0; j < 6; ++j)
+        atomicAdd(&H[(l0 + i) * n + l0 + j], J[j0 + i] * J[j0 + j] + J[12 + j0 + i] * J[12 + j0 + j] + J[24 + j0 + i] * J[24 + j0 + j]);
+    }
+  }
+}
+// dense path: the full J^T J (pose-sensor cross block included) into the lower triangle of S (element (i, j), i >= j, at
+// Sd[j * nc + i])
+__global__ void ba_prior_dense_kernel(const BaDev D, const BaPrior P) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= P.n) return;
+  const int4 ix = P.idx[k];
+  const double* J = P.J + 36 * (long long)k;
+  for (int a = 0; a < 12; ++a) {
+    const int ia = ba_prior_col(ix, a);
+    if (ia < 0) continue;
+    for (int b = 0; b < 12; ++b) {
+      const int ib = ba_prior_col(ix, b);
+      if (ib >= 0 && ia >= ib) atomicAdd(&D.Sd[(long long)ib * D.nc + ia], J[a] * J[b] + J[12 + a] * J[12 + b] + J[24 + a] * J[24 + b]);
+    }
+  }
+}
+// PCG: q += J^T (J p) after the observations' SpMV
+__global__ void ba_prior_spmv_kernel(const BaDev D, const BaPrior P) {
+  if (D.ctl->done) return;
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= P.n) return;
+  const int4 ix = P.idx[k];
+  const double* J = P.J + 36 * (long long)k;
+  double y[3] = {0.0, 0.0, 0.0};
+  for (int j = 0; j < 12; ++j) {
+    const int col = ba_prior_col(ix, j);
+    if (col < 0) continue;
+    const double v = D.p[col];
+    for (int a = 0; a < 3; ++a) y[a] += J[12 * a + j] * v;
+  }
+  for (int j = 0; j < 12; ++j) {
+    const int col = ba_prior_col(ix, j);
+    if (col >= 0) atomicAdd(&D.q[col], J[j] * y[0] + J[12 + j] * y[1] + J[24 + j] * y[2]);
+  }
+}
+// the candidate: model decrease -(J d)^T (r + J d / 2) of the prior rows, their cost at the candidate parameters and
+// rho(new) - rho(old) prior by prior
+__global__ void __launch_bounds__(BA_BLOCK) ba_prior_step_kernel(const BaDev D, const BaPrior P) {
+  __shared__ double sm[8];
+  const int k = blockIdx.x * BA_BLOCK + threadIdx.x;
+  double model = 0.0, cost = 0.0, delta = 0.0;
+  if (k < P.n) {
+    const int4 ix = P.idx[k];
+    const double* J = P.J + 36 * (long long)k;
+    const double* r = P.r + 3 * (long long)k;
+    double y[3] = {0.0, 0.0, 0.0};
+    for (int j = 0; j < 12; ++j) {
+      const int col = ba_prior_col(ix, j);
+      if (col < 0) continue;
+      const double v = D.x[col];
+      for (int a = 0; a < 3; ++a) y[a] += J[12 * a + j] * v;
+    }
+    model = -(y[0] * (r[0] + 0.5 * y[0]) + y[1] * (r[1] + 0.5 * y[1]) + y[2] * (r[2] + 0.5 * y[2]));
+    double rw[3], rho[3];
+    ba_prior_eval(D, P, k, D.nposes_, D.nsensors_, rw, nullptr);
+    ba_loss(P.loss_type, P.loss_scale, rw[0] * rw[0] + rw[1] * rw[1] + rw[2] * rw[2], rho);
+    cost = 0.5 * rho[0];
+    delta = cost - P.cost[k];
+  }
+  double t = ba_block_sum(model, sm);
+  if (threadIdx.x == 0) atomicAdd(&D.ctl->model, t);
+  t = ba_block_sum(cost, sm);
+  if (threadIdx.x == 0) atomicAdd(&D.ctl->new_cost, t);
+  t = ba_block_sum(delta, sm);
+  if (threadIdx.x == 0) atomicAdd(&D.ctl->cost_delta, t);
+}
+// Host checks of the caller's priors, before any device work: indices, finite values, SPD covariances.  W receives the
+// weights of all priors.
+static int ba_prior_check(const b200ba_problem* p, const b200ba_position_priors* pr, std::vector<double>& W) {
+  if (pr->num_priors < 0) return ba_fail(-2, "num_priors < 0");
+  if (pr->num_priors && (!pr->pose_idx || !pr->position || !pr->covariance)) return ba_fail(-1, "null prior array");
+  const int t = pr->loss_function_type;
+  if (t != B200BA_LOSS_TRIVIAL && t != B200BA_LOSS_SOFT_L1 && t != B200BA_LOSS_CAUCHY && t != B200BA_LOSS_HUBER)
+    return ba_fail(-2, "unknown prior loss function type");
+  if (t != B200BA_LOSS_TRIVIAL && !(pr->loss_function_scale > 0.0 && std::isfinite(pr->loss_function_scale)))
+    return ba_fail(-2, "prior loss function scale must be positive and finite");
+  W.assign(9 * (size_t)pr->num_priors, 0.0);
+  for (int k = 0; k < pr->num_priors; ++k) {
+    const std::string at = "prior " + std::to_string(k) + ": ";
+    if (pr->pose_idx[k] < 0 || pr->pose_idx[k] >= p->num_poses) return ba_fail(-2, at + "pose_idx out of range");
+    const int s = pr->sensor_idx ? pr->sensor_idx[k] : -1;
+    if (s < -1 || s >= p->num_sensors) return ba_fail(-2, at + "sensor_idx out of range");
+    for (int a = 0; a < 3; ++a) if (!std::isfinite(pr->position[3 * (size_t)k + a])) return ba_fail(-2, at + "position is not finite");
+    for (int a = 0; a < 9; ++a) if (!std::isfinite(pr->covariance[9 * (size_t)k + a])) return ba_fail(-2, at + "covariance is not finite");
+    if (!ba_prior_weight(pr->covariance + 9 * (size_t)k, W.data() + 9 * (size_t)k)) return ba_fail(-2, at + "covariance is not symmetric positive definite");
+  }
+  return 0;
+}
+// The priors the solve keeps (a pose or sensor block of theirs is variable), uploaded; returns their number in P.n.
+static int ba_prior_setup(const b200ba_position_priors* pr, const std::vector<double>& W, const BaLayout& L, BaPool& pool,
+                          cudaStream_t st, BaPrior& P) {
+  std::vector<int4> idx;
+  std::vector<double> c, w;
+  for (int k = 0; k < pr->num_priors; ++k) {
+    const int pi = pr->pose_idx[k], si = pr->sensor_idx ? pr->sensor_idx[k] : -1;
+    const int cam = si >= 0 ? L.sens_cam[si] : -1;
+    const int po = L.pose_off[pi], so = (cam >= 0 && L.cam_ns[cam] == 6) ? L.cam_off[cam] : -1;
+    if (po < 0 && so < 0) continue;   // all its blocks constant (bundle_adjustment_ceres.cc:992-1000)
+    idx.push_back(make_int4(pi, si, po, so));
+    c.insert(c.end(), pr->position + 3 * (size_t)k, pr->position + 3 * (size_t)k + 3);
+    w.insert(w.end(), W.begin() + 9 * (size_t)k, W.begin() + 9 * (size_t)k + 9);
+  }
+  P.n = (int)idx.size();
+  P.loss_type = pr->loss_function_type; P.loss_scale = pr->loss_function_scale;
+  if (!P.n) return 0;
+  BA_CUDA(pool.upload(&P.idx, idx, st)); BA_CUDA(pool.upload(&P.c, c, st)); BA_CUDA(pool.upload(&P.W, w, st));
+  BA_CUDA(pool.alloc(&P.J, 36 * (size_t)P.n)); BA_CUDA(pool.alloc(&P.r, 3 * (size_t)P.n)); BA_CUDA(pool.alloc(&P.cost, (size_t)P.n));
+  return 0;
+}
+
 // ---- the LM loop ----
 // B200BA_PROFILE=1: device-timeline breakdown of the solve by phase (events between the launches; the interval that
 // ends at a "host" mark is GPU idle time spent waiting for the host round trip).  Diagnostic only.
@@ -3134,6 +3411,7 @@ struct BaSolve {
   BaReducer red;
   BaPath path;
   BaDev D;
+  BaPrior P;                 // position priors (P.n = 0: none)
   int pack = 0, dkmax = 0;   // packed size of the camera-side blocks, widest camera block
   const bool check = getenv("B200BA_CHECK") != nullptr;   // synchronise and test for asynchronous errors after every group of launches
   const bool profile = getenv("B200BA_PROFILE") != nullptr;
@@ -3160,6 +3438,7 @@ struct BaSolve {
   }
   unsigned gc_blocks() const { return (unsigned)((D.nc + 255) / 256); }
   unsigned gp_blocks() const { return (unsigned)((D.nvpt + 255) / 256); }
+  unsigned prior_blocks() const { return (unsigned)((P.n + 255) / 256); }
   bool replica() const { return red.comm && red.comm->rank != 0; }   // sharded, not rank 0: replicated terms come from rank 0
   cudaError_t zero(void* field, size_t bytes = sizeof(double)) { return cudaMemsetAsync(field, 0, bytes, st); }
   cudaError_t read_ctl() { cudaError_t e = cudaMemcpyAsync(h, D.ctl, sizeof(BaCtl), cudaMemcpyDeviceToHost, st); if (e != cudaSuccess) return e; return cudaStreamSynchronize(st); }
@@ -3172,6 +3451,7 @@ struct BaSolve {
   int linearize(int apply_scale) {
     BA_CUDA(zero(&D.ctl->cost));
     BA_DISPATCH_DC(ba_launch_linearize, D, apply_scale, st);
+    if (P.n) { ba_prior_linearize_kernel<<<prior_blocks(), BA_BLOCK, 0, st>>>(D, P, apply_scale); ++launches; }
     mark(PF_LIN);
     BA_CUDA(red(&D.ctl->cost, 1, ncclDouble, ncclSum));
     mark(PF_AR_COST);
@@ -3185,6 +3465,7 @@ struct BaSolve {
     BA_CUDA(zero(D.scale_c, sizeof(double) * (D.nc ? D.nc : 1)));
     BA_CUDA(zero(D.scale_p, sizeof(double) * (D.nvpt ? 3 * (size_t)D.nvpt : 1)));
     ba_colnorm_kernel<<<D.nblocks, BA_BLOCK, 0, st>>>(D);
+    if (P.n) { ba_prior_colnorm_kernel<<<prior_blocks(), 256, 0, st>>>(D, P); ++launches; }   // ceres scales over every residual row
     BA_CUDA(red(D.scale_c, D.nc, ncclDouble, ncclSum));
     if (D.nc) ba_make_scale_kernel<<<gc_blocks(), 256, 0, st>>>(D.scale_c, D.nc, o->jacobi_scaling);
     if (D.nvpt) ba_make_scale_kernel<<<(3 * D.nvpt + 255) / 256, 256, 0, st>>>(D.scale_p, 3LL * D.nvpt, o->jacobi_scaling);
@@ -3202,6 +3483,7 @@ struct BaSolve {
     BA_TRY(checkpoint("build_cam_sorted"));
     if (D.nchunks_off) ba_cam_offdiag_kernel<false><<<(D.nchunks_off + BA_SC_BLOCK / 32 - 1) / (BA_SC_BLOCK / 32), BA_SC_BLOCK, 0, st>>>(D);
     BA_TRY(checkpoint("cam_offdiag<false>"));
+    if (P.n) { ba_prior_build_kernel<<<prior_blocks(), 256, 0, st>>>(D, P); ++launches; }   // before the LM diagonal and gmax read them
     mark(PF_BUILD);
     red.begin();
     BA_CUDA(red(D.gc, D.nc, ncclDouble, ncclSum));
@@ -3254,7 +3536,7 @@ struct BaSolve {
     BA_CUDA(zero(D.ctl, offsetof(BaCtl, iters_total)));  // keeps iters_total
     BA_CUDA(cudaMemcpyAsync(&D.ctl->cost, &cost, sizeof(double), cudaMemcpyHostToDevice, st));
     if (!D.nc || path.dense) {
-      if (D.nc) { BA_DISPATCH_DC(ba_launch_dense, D, st); launches += 3; }
+      if (D.nc) { BA_DISPATCH_DC(ba_launch_dense, D, P, st); launches += 3 + (P.n ? 1 : 0); }
       if (read) BA_CUDA(read_ctl());
       return 0;
     }
@@ -3278,6 +3560,7 @@ struct BaSolve {
         if (b == 0) BA_CUDA(cudaEventRecord(ev[2], st));  // first SpMV of a batch always does real work
         BA_DISPATCH_DC(ba_launch_spmv, D, path, st);
         if (b == 0) BA_CUDA(cudaEventRecord(ev[3], st));
+        if (P.n) { ba_prior_spmv_kernel<<<prior_blocks(), 256, 0, st>>>(D, P); ++launches; }   // q += J^T J p of the prior rows
         mark(PF_SPMV);
         BA_CUDA(red(D.q, D.nc, ncclDouble, ncclSum, &D.ctl->done));  // the one data-path collective of a PCG iteration
         mark(PF_AR_Q);
@@ -3310,6 +3593,7 @@ struct BaSolve {
     BA_CUDA(zero(&D.ctl->cost_delta));
     if (D.wide) ba_cost_kernel<true><<<D.nblocks, BA_BLOCK, 0, st>>>(D, D.nposes_, D.ncams_, D.npts_, D.nsensors_, &D.ctl->new_cost);
     else ba_cost_kernel<false><<<D.nblocks, BA_BLOCK, 0, st>>>(D, D.nposes_, D.ncams_, D.npts_, D.nsensors_, &D.ctl->new_cost);
+    if (P.n) { ba_prior_step_kernel<<<prior_blocks(), BA_BLOCK, 0, st>>>(D, P); ++launches; }
     BA_TRY(checkpoint("update + cost"));
     mark(PF_UPDATE_COST);
     BA_CUDA(red(&D.ctl->new_cost, 3, ncclDouble, ncclSum));   // new_cost, model, cost_delta are adjacent in BaCtl
@@ -3337,10 +3621,14 @@ static int ba_write_back(const BaLayout& L, const BaDev& D, b200ba_problem* p) {
   for (long long i = 0; i < NPT; ++i) if (L.pt_var[i] >= 0) memcpy(p->points + 3 * i, h_pts.data() + 3 * i, 24);
   return 0;
 }
-static int ba_solve_impl(const b200ba_options* o, b200ba_problem* p, b200ba_summary* sum, b200ba_comm* comm) {
+static int ba_solve_impl(const b200ba_options* o, b200ba_problem* p, b200ba_summary* sum, b200ba_comm* comm,
+                         const b200ba_position_priors* priors) {
   if (!o || !p || !sum) return ba_fail(-1, "null argument");
   memset(sum, 0, sizeof(*sum));
   sum->termination_type = B200BA_FAILURE;
+  if (priors && priors->num_priors == 0) priors = nullptr;
+  std::vector<double> prior_w;   // checked before any device work
+  if (priors) BA_TRY(ba_prior_check(p, priors, prior_w));
   BaPool pool;
   const auto t_setup0 = std::chrono::steady_clock::now();
   int ndev = 0;
@@ -3360,6 +3648,10 @@ static int ba_solve_impl(const b200ba_options* o, b200ba_problem* p, b200ba_summ
   S.pack = L.pack; S.dkmax = L.dkmax;
   BA_TRY(ba_select_path(o, L, red.comm != nullptr, red.sms, S.path));
   BA_TRY(ba_upload(L, o, p, S.path, red.comm, pool, S.st, S.D));
+  if (priors) {
+    BA_TRY(ba_prior_setup(priors, prior_w, L, pool, S.st, S.P));
+    sum->num_residuals += 3 * S.P.n;
+  }
   sum->setup_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_setup0).count();
 
   for (int i = 0; i < 4; ++i) BA_CUDA(cudaEventCreate(&S.ev[i]));
@@ -3507,6 +3799,24 @@ int b200ba_test_pack(const b200ba_options* o, b200ba_problem* p, int64_t capacit
   memcpy(vpt_s1, L.vpt_s1.data(), sizeof(int) * L.vpt_s1.size());
   memcpy(vpt_point, L.vpt_point.data(), sizeof(int) * L.vpt_point.size());
   return 0;
+}
+
+// ---- position priors (include/b200_ba_pose_prior.h) ----
+void b200ba_position_priors_init(b200ba_position_priors* p) {
+  memset(p, 0, sizeof(*p));
+  p->loss_function_type = B200BA_LOSS_TRIVIAL;
+  p->loss_function_scale = 2.7954834829151074;   // sqrt(7.814727903251179), the chi-square 95 % quantile of 3 DoF
+}
+int b200ba_solve_with_position_priors(const b200ba_options* o, b200ba_problem* p, const b200ba_position_priors* priors,
+                                      b200ba_summary* out) {
+  return ba_solve_impl(o, p, out, nullptr, priors);
+}
+void b200ba_test_prior_position(const double* rig, const double* sensor, const double* position, double* res,
+                                double* J_rig, double* J_sensor) {
+  ba_prior_position(rig, sensor, position, res, J_rig, J_sensor);
+}
+int b200ba_test_prior_weight(const double* covariance, double* weight) {
+  return ba_prior_weight(covariance, weight) ? 0 : ba_fail(-2, "covariance is not symmetric positive definite");
 }
 
 }  // extern "C"

@@ -431,11 +431,13 @@ def synthesize_rig_problem(num_frames, num_sensors, num_points, track_length, mo
 
 
 def synthesize_rig_reconstruction(num_rigs, num_cameras_per_rig, num_frames_per_rig, num_points3D, model=2, seed=0,
-                                  point2D_stddev=0.0):
+                                  point2D_stddev=0.0, prior_position=False):
     """SynthesizeDataset with rigs (scene/synthetic.cc:341-672) as a Reconstruction of the Python mirror: `num_rigs` rigs of
     `num_cameras_per_rig` cameras each (own intrinsics; the first camera of a rig is its reference sensor), every rig
     with `num_frames_per_rig` frames, one image per (frame, sensor), image / camera / frame / rig ids ascending from 1 in
-    that order, every point observed by every image (as in the reference's small test scenes)."""
+    that order, every point observed by every image (as in the reference's small test scenes).  prior_position=True
+    returns (rec, pose_priors) with one PosePrior per image at its projection centre and no covariance
+    (scene/synthetic.cc:497-523); synthesize_noise perturbs them."""
     from .bundle_adjustment import Camera, Frame, Image, MODEL_NUM_PARAMS, Point2D, Point3D, Reconstruction, Rig, _rigid_compose
     rng = np.random.default_rng(seed)
     rec = Reconstruction()
@@ -475,5 +477,42 @@ def synthesize_rig_reconstruction(num_rigs, num_cameras_per_rig, num_frames_per_
                     im.points2D.append(Point2D(xy[k].copy(), k + 1))
                     rec.points3D[k + 1].track.append((img_id, k))
                 rec.images[img_id] = im
+    if prior_position:
+        from .bundle_adjustment import PosePrior, projection_center
+        return rec, [PosePrior(i, projection_center(rec, i)) for i in sorted(rec.images)]
+    return rec
+
+
+def synthesize_noise(rec, pose_priors=None, point2D_stddev=0.0, point3D_stddev=0.0, rig_from_world_rotation_stddev=0.0,
+                     rig_from_world_translation_stddev=0.0, prior_position_stddev=0.0, seed=1):
+    """SynthesizeNoise (scene/synthetic.cc:675-768) on a reconstruction with frames, in place: Gaussian pixel and point
+    noise, rig_from_world rotation noise (degrees, about a random axis) and translation noise, and Gaussian noise on the
+    prior positions with covariance prior_position_stddev^2 I (the covariance is set even for a zero stddev only when
+    pose_priors are given and the stddev is positive)."""
+    from .bundle_adjustment import _rigid_compose
+    rng = np.random.default_rng(seed)
+    for f in sorted(rec.frames):
+        fr = rec.frames[f]
+        if rig_from_world_rotation_stddev > 0:
+            ax = rng.normal(size=3); ax /= np.linalg.norm(ax)
+            a = np.deg2rad(rng.normal(0, rig_from_world_rotation_stddev))
+            dq = np.concatenate([ax * np.sin(a / 2), [np.cos(a / 2)]])
+            fr.rig_from_world[:4] = _quat_mul(dq[None], fr.rig_from_world[None, :4])[0]
+        if rig_from_world_translation_stddev > 0:
+            fr.rig_from_world[4:] += rng.normal(0, rig_from_world_translation_stddev, 3)
+    for im in rec.images.values():   # keep the derived image poses in step with the frames
+        fr = rec.frames[im.frame_id]
+        rig = rec.rigs[fr.rig_id]
+        im.cam_from_world[:] = fr.rig_from_world if rig.ref_sensor == im.camera_id else _rigid_compose(rig.sensors[im.camera_id], fr.rig_from_world)
+        if point2D_stddev > 0:
+            for p2 in im.points2D:
+                p2.xy = p2.xy + rng.normal(0, point2D_stddev, 2)
+    if point3D_stddev > 0:
+        for k in sorted(rec.points3D):
+            rec.points3D[k].xyz += rng.normal(0, point3D_stddev, 3)
+    if pose_priors is not None and prior_position_stddev > 0:
+        for pp in pose_priors:
+            pp.position = pp.position + rng.normal(0, prior_position_stddev, 3)
+            pp.position_covariance = prior_position_stddev ** 2 * np.eye(3)
     return rec
 
