@@ -853,6 +853,9 @@ def _bind_cov(lib):
     vp, i64 = ctypes.c_void_p, ctypes.c_int64
     lib.b200ba_estimate_covariance.argtypes = [ctypes.POINTER(_COptions), ctypes.POINTER(_CCovOptions), ctypes.POINTER(_CProblem),
                                                ctypes.POINTER(vp)]
+    lib.b200ba_estimate_covariance_with_position_priors.argtypes = [
+        ctypes.POINTER(_COptions), ctypes.POINTER(_CCovOptions), ctypes.POINTER(_CProblem), ctypes.POINTER(_CPositionPriors),
+        ctypes.POINTER(vp)]
     lib.b200ba_covariance_point.argtypes = [vp, i64, _f64p]
     lib.b200ba_covariance_pose.argtypes = [vp, ctypes.c_int, _f64p]
     lib.b200ba_covariance_pose_cross.argtypes = [vp, ctypes.c_int, ctypes.c_int, _f64p, _i32p, _i32p]
@@ -936,18 +939,25 @@ class CovarianceNotEstimable(BundleAdjustmentError):
 
 
 def estimate_covariance_flat(options: BundleAdjustmentOptions, cov_options: BACovarianceOptions, flat: FlatProblem,
-                             raise_not_estimable=False):
-    """b200ba_estimate_covariance on a flat problem (rigs included).  Returns a FlatCovariance, or None when the reduced
+                             raise_not_estimable=False, priors: Optional["FlatPositionPriors"] = None):
+    """b200ba_estimate_covariance on a flat problem (rigs included), or, with `priors` (FlatPositionPriors in the frame
+    of `flat`), b200ba_estimate_covariance_with_position_priors.  Returns a FlatCovariance, or None when the reduced
     matrix is rank deficient (raise_not_estimable: raise CovarianceNotEstimable with the library's message instead)."""
     lib = _bind_cov(_bind(load_library()))
     co, cc, cp, h = options.to_c(), _CCovOptions(int(cov_options.params), float(cov_options.damping)), flat.to_c(), ctypes.c_void_p()
-    rc = lib.b200ba_estimate_covariance(ctypes.byref(co), ctypes.byref(cc), ctypes.byref(cp), ctypes.byref(h))
+    if priors is None:
+        name = "b200ba_estimate_covariance"
+        rc = lib.b200ba_estimate_covariance(ctypes.byref(co), ctypes.byref(cc), ctypes.byref(cp), ctypes.byref(h))
+    else:
+        name, cpr = "b200ba_estimate_covariance_with_position_priors", priors.to_c()
+        rc = lib.b200ba_estimate_covariance_with_position_priors(ctypes.byref(co), ctypes.byref(cc), ctypes.byref(cp),
+                                                                  ctypes.byref(cpr), ctypes.byref(h))
     if rc == 1:
         if raise_not_estimable:
             raise CovarianceNotEstimable(lib.b200ba_last_error().decode())
         return None
     if rc != 0:
-        raise BundleAdjustmentError(f"b200ba_estimate_covariance failed ({rc}): {lib.b200ba_last_error().decode()}")
+        raise BundleAdjustmentError(f"{name} failed ({rc}): {lib.b200ba_last_error().decode()}")
     return FlatCovariance(lib, h.value, len(flat.poses), len(flat.points))
 
 
@@ -1043,17 +1053,19 @@ class BACovariance:
 
 def EstimateBACovariance(options: BACovarianceOptions, reconstruction: Reconstruction, bundle_adjuster: BundleAdjuster):
     """EstimateBACovariance (covariance.cc): the covariance of the problem `bundle_adjuster` solves, at the parameters
-    the reconstruction holds now (call it after Solve()).  None when the problem is not estimable (unfixed gauge)."""
+    the reconstruction holds now (call it after Solve()).  None when the problem is not estimable (unfixed gauge).
+    A PosePriorBundleAdjuster's prior residuals are part of the problem, taken in the frame the reconstruction is in
+    (normalized after the constructor, metric after Solve())."""
     rec = reconstruction
-    if isinstance(bundle_adjuster, PosePriorBundleAdjuster):
-        raise BundleAdjustmentError("EstimateBACovariance of a pose-prior bundle adjustment is not supported: the covariance "
-                                    "would ignore the prior residuals")
     for image_id in rec.images:
         if not rec.IsRefInFrame(image_id):
             raise BundleAdjustmentError(f"image {image_id} is not the reference sensor of its frame: pose covariances of "
                                         "non-trivial frames are not supported")
     flat, pose_ids, camera_ids, point_ids = bundle_adjuster.flat_problem()
-    cov = estimate_covariance_flat(bundle_adjuster.Options(), options, flat)
+    priors = None
+    if isinstance(bundle_adjuster, PosePriorBundleAdjuster):
+        priors = bundle_adjuster.flat_priors(flat, pose_ids, normalized=bundle_adjuster.in_normalized_frame_)
+    cov = estimate_covariance_flat(bundle_adjuster.Options(), options, flat, priors=priors)
     if cov is None:
         return None
     if rec.frames:      # pose k = frame k; every image is its frame's reference sensor
@@ -1414,14 +1426,19 @@ class PosePriorBundleAdjuster(BundleAdjuster):
             self.normalized_from_metric_ = normalize_reconstruction(reconstruction, fixed_scale=True)
         else:
             config.FixGauge(TWO_CAMS_FROM_WORLD)
+        # the frame the reconstruction is in: normalized until Solve() transforms it back to the metric frame
+        self.in_normalized_frame_ = self.use_prior_position_
 
-    def flat_priors(self, flat: FlatProblem, pose_ids) -> FlatPositionPriors:
-        """The priors of the parameterized images, in the normalized frame, indexed into `flat` (AddImagePosePriorToProblem,
-        bundle_adjustment_ceres.cc:987-1039; the library skips those whose blocks are all constant)."""
+    def flat_priors(self, flat: FlatProblem, pose_ids, normalized=True) -> FlatPositionPriors:
+        """The priors of the parameterized images, indexed into `flat` (AddImagePosePriorToProblem,
+        bundle_adjustment_ceres.cc:987-1039; the library skips those whose blocks are all constant).  normalized: in the
+        normalized frame the solve runs in; else in the metric frame of the priors as given.  Empty when the adjuster
+        fell back to the TWO_CAMS_FROM_WORLD gauge."""
         rec, po = self.reconstruction_, self.prior_options_
         pose_index = {p: k for k, p in enumerate(pose_ids)}
         sensor_of_cam = {c: k for k, c in enumerate(getattr(flat, "sensor_camera_ids", []))}
-        sR = self.normalized_from_metric_.scale * self.normalized_from_metric_.R()
+        to_frame = self.normalized_from_metric_ if normalized else Sim3d()
+        sR = to_frame.scale * to_frame.R()
         pose_idx, sensor_idx, pos, cov = [], [], [], []
         if self.use_prior_position_:
             for pp in self.pose_priors_:
@@ -1430,7 +1447,7 @@ class PosePriorBundleAdjuster(BundleAdjuster):
                 im = rec.images[pp.image_id]
                 pose_idx.append(pose_index[im.frame_id if rec.frames else pp.image_id])
                 sensor_idx.append(-1 if rec.IsRefInFrame(pp.image_id) else sensor_of_cam[im.camera_id])
-                pos.append(self.normalized_from_metric_ * pp.position)
+                pos.append(to_frame * pp.position)
                 C = pp.position_covariance if pp.HasPositionCov() else po.prior_position_fallback_stddev ** 2 * np.eye(3)
                 cov.append(sR @ C @ sR.T)
         return FlatPositionPriors(pose_idx, sensor_idx, np.reshape(pos, (-1, 3)), np.reshape(cov, (-1, 3, 3)),
@@ -1442,6 +1459,7 @@ class PosePriorBundleAdjuster(BundleAdjuster):
     def Solve(self) -> BundleAdjustmentSummary:
         summary = super().Solve()
         transform_reconstruction(self.reconstruction_, self.normalized_from_metric_.inverse())
+        self.in_normalized_frame_ = False
         return summary
 
 

@@ -3219,6 +3219,26 @@ __device__ __forceinline__ void ba_prior_eval(const BaDev& D, const BaPrior& P, 
 }
 // camera-side offset of column j of a prior's Jacobian, or -1
 __device__ __forceinline__ int ba_prior_col(const int4& ix, int j) { return j < 6 ? (ix.z >= 0 ? ix.z + j : -1) : (ix.w >= 0 ? ix.w + j - 6 : -1); }
+// ceres Corrector of the priors' loss (rho at sq = |rw|^2) applied to the weighted 3 x 12 Jacobian J in place; returns
+// the factor of the corrected residual
+__device__ __forceinline__ double ba_prior_correct(const BaPrior& P, const double* rw, double sq, const double* rho, double* J) {
+  double rs = 1.0;
+  if (P.loss_type != B200BA_LOSS_TRIVIAL) {
+    const double sqrt_rho1 = sqrt(rho[1]);
+    double alpha_sq_norm = 0.0;
+    rs = sqrt_rho1;
+    if (sq != 0.0 && rho[2] > 0.0) {
+      const double alpha = 1.0 - sqrt(1.0 + 2.0 * sq * rho[2] / rho[1]);
+      rs = sqrt_rho1 / (1 - alpha);
+      alpha_sq_norm = alpha / sq;
+    }
+    for (int j = 0; j < 12; ++j) {
+      const double rj = rw[0] * J[j] + rw[1] * J[12 + j] + rw[2] * J[24 + j];
+      for (int a = 0; a < 3; ++a) J[12 * a + j] = sqrt_rho1 * (J[12 * a + j] - alpha_sq_norm * rw[a] * rj);
+    }
+  }
+  return rs;
+}
 // linearisation: residual, Jacobian (ceres Corrector with the priors' loss, Jacobi scaling when apply_scale), cost
 __global__ void __launch_bounds__(BA_BLOCK) ba_prior_linearize_kernel(const BaDev D, const BaPrior P, int apply_scale) {
   __shared__ double sm[8];
@@ -3230,21 +3250,7 @@ __global__ void __launch_bounds__(BA_BLOCK) ba_prior_linearize_kernel(const BaDe
     const double sq = rw[0] * rw[0] + rw[1] * rw[1] + rw[2] * rw[2];
     ba_loss(P.loss_type, P.loss_scale, sq, rho);
     cost = 0.5 * rho[0];
-    double rs = 1.0;
-    if (P.loss_type != B200BA_LOSS_TRIVIAL) {
-      const double sqrt_rho1 = sqrt(rho[1]);
-      double alpha_sq_norm = 0.0;
-      rs = sqrt_rho1;
-      if (sq != 0.0 && rho[2] > 0.0) {
-        const double alpha = 1.0 - sqrt(1.0 + 2.0 * sq * rho[2] / rho[1]);
-        rs = sqrt_rho1 / (1 - alpha);
-        alpha_sq_norm = alpha / sq;
-      }
-      for (int j = 0; j < 12; ++j) {
-        const double rj = rw[0] * J[j] + rw[1] * J[12 + j] + rw[2] * J[24 + j];
-        for (int a = 0; a < 3; ++a) J[12 * a + j] = sqrt_rho1 * (J[12 * a + j] - alpha_sq_norm * rw[a] * rj);
-      }
-    }
+    const double rs = ba_prior_correct(P, rw, sq, rho, J);
     const int4 ix = P.idx[k];
     for (int j = 0; j < 12; ++j) {
       const int col = ba_prior_col(ix, j);
@@ -3932,6 +3938,31 @@ __global__ void __launch_bounds__(BA_BLOCK) ba_cov_point_kernel(const BaDev D, c
     }
   }
 }
+// Position priors (b200ba_estimate_covariance_with_position_priors): S += J^T J of each kept prior's weighted,
+// loss-corrected, unscaled 3 x 12 rows [pose | sensor], fp64, one thread per prior.  The rows touch camera-side blocks
+// only (pose, pose-sensor cross terms, sensor), so the point elimination above is unaffected.  The solve's
+// ba_prior_linearize_kernel is not reused: it applies Jacobi scaling and sums the cost into the LM control block.
+__global__ void ba_cov_prior_kernel(const BaDev D, const BaPrior P, const BaCov C) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= P.n) return;
+  double rw[3], J[36], rho[3];
+  ba_prior_eval(D, P, k, D.poses, D.sensors, rw, J);
+  const double sq = rw[0] * rw[0] + rw[1] * rw[1] + rw[2] * rw[2];
+  ba_loss(P.loss_type, P.loss_scale, sq, rho);
+  ba_prior_correct(P, rw, sq, rho, J);
+  const int4 ix = P.idx[k];
+  int row[12];
+  for (int j = 0; j < 12; ++j) {
+    const int col = ba_prior_col(ix, j);
+    row[j] = col >= 0 ? C.colmap[col] : -1;
+  }
+  for (int a = 0; a < 12; ++a) {
+    if (row[a] < 0) continue;
+    for (int b = 0; b < 12; ++b)
+      if (row[b] >= 0 && row[a] >= row[b])
+        atomicAdd(&C.S[(long long)row[b] * C.N + row[a]], J[a] * J[b] + J[12 + a] * J[12 + b] + J[24 + a] * J[24 + b]);
+  }
+}
 // diagonal: damping on rows [0, n_damp) (the others, eliminated in POSES mode), 1 on the padding rows [n, N)
 __global__ void ba_cov_diag_kernel(double* S, long long N, int n, int n_damp, double damping) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -3980,11 +4011,16 @@ static std::string ba_cov_row_name(const b200ba_covariance& H, int r) {
     if (H.sens_size[i] && r >= H.sens_row[i] && r < H.sens_row[i] + H.sens_size[i]) { snprintf(b, sizeof(b), "sensor_from_rig %zu, tangent row %d", i, r - H.sens_row[i]); return b; }
   return "padding";
 }
-static int ba_cov_impl(const b200ba_options* o, const b200ba_covariance_options* co, const b200ba_problem* p, b200ba_covariance_t* out) {
+// priors: the position priors the problem was solved with (PosePriorBundleAdjuster), or null
+static int ba_cov_impl(const b200ba_options* o, const b200ba_covariance_options* co, const b200ba_problem* p,
+                       const b200ba_position_priors* priors, b200ba_covariance_t* out) {
   if (!o || !co || !p || !out) return ba_fail(-1, "null argument");
   *out = nullptr;
   if (co->params < B200BA_COV_POSES || co->params > B200BA_COV_ALL) return ba_fail(-2, "unknown covariance mode");
   if (!(co->damping >= 0.0)) return ba_fail(-2, "damping must be >= 0");
+  if (priors && priors->num_priors == 0) priors = nullptr;
+  std::vector<double> prior_w;   // checked before any device work
+  if (priors) BA_TRY(ba_prior_check(p, priors, prior_w));
   const auto t0 = std::chrono::steady_clock::now();
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return ba_fail(-101, "no CUDA device: colmap_b200 has no CPU fallback");
@@ -4036,6 +4072,8 @@ static int ba_cov_impl(const b200ba_options* o, const b200ba_covariance_options*
   BaPath path = {};       // no reduced-system path: only the layout and the slot arrays are used
   BaDev D;
   BA_TRY(ba_upload(L, o, p, path, nullptr, work, G.st, D));
+  BaPrior P;              // the priors only enter S: none are set up when S is not formed (POINTS mode)
+  if (priors && n) BA_TRY(ba_prior_setup(priors, prior_w, L, work, G.st, P));
   BaCov C = {};
   C.damping = co->damping; C.want_S = n > 0; C.N = N;
   BA_CUDA(work.alloc(&C.J, (size_t)(2 * L.DC + 6) * (size_t)D.nslots));
@@ -4052,6 +4090,7 @@ static int ba_cov_impl(const b200ba_options* o, const b200ba_covariance_options*
   H->ms[0] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
   BA_CUDA(cudaEventRecord(G.ev[0], G.st));
   BA_DISPATCH_DC(ba_cov_launch_build, D, C, G.st);
+  if (P.n) ba_cov_prior_kernel<<<(P.n + 127) / 128, 128, 0, G.st>>>(D, P, C);
   if (n) ba_cov_diag_kernel<<<(unsigned)((N + 255) / 256), 256, 0, G.st>>>(C.S, N, n, want_others ? 0 : n_others, co->damping);
   BA_CUDA(cudaGetLastError());
   BA_CUDA(cudaEventRecord(G.ev[1], G.st));
@@ -4128,7 +4167,12 @@ void b200ba_covariance_options_init(b200ba_covariance_options* c) { c->params = 
 
 int b200ba_estimate_covariance(const b200ba_options* o, const b200ba_covariance_options* c, const b200ba_problem* p,
                                b200ba_covariance_t* out) {
-  return ba_cov_impl(o, c, p, out);
+  return ba_cov_impl(o, c, p, nullptr, out);
+}
+int b200ba_estimate_covariance_with_position_priors(const b200ba_options* o, const b200ba_covariance_options* c,
+                                                    const b200ba_problem* p, const b200ba_position_priors* priors,
+                                                    b200ba_covariance_t* out) {
+  return ba_cov_impl(o, c, p, priors, out);
 }
 
 int b200ba_covariance_point(b200ba_covariance_t h, int64_t point, double out[9]) {

@@ -7,6 +7,7 @@
 #define B200_BA_COVARIANCE_H_
 
 #include "b200_bundle_adjustment.h"
+#include "b200_ba_pose_prior.h"
 
 #ifdef __cplusplus
 extern "C" {
@@ -31,6 +32,15 @@ typedef struct b200ba_covariance* b200ba_covariance_t;
  * names the block and the pivot, *out stays NULL), < 0 = error. */
 int b200ba_estimate_covariance(const b200ba_options* o, const b200ba_covariance_options* c, const b200ba_problem* p,
                                b200ba_covariance_t* out);
+/* The same for a problem solved with b200ba_solve_with_position_priors (the reference's EstimateBACovariance on a
+ * PosePriorBundleAdjuster): J also holds the covariance-weighted prior rows, corrected by the priors' own loss, so the
+ * priors can make S invertible where no gauge is fixed.  The priors are read at the parameters of p and must be in the
+ * same frame.  Priors whose blocks are all constant are skipped; they never touch the point blocks.  Bad priors (index
+ * out of range, non-finite values, a covariance that is not SPD) return < 0 with a message before any device work.
+ * priors == NULL or num_priors == 0 is b200ba_estimate_covariance.  Return codes and the handle as above. */
+int b200ba_estimate_covariance_with_position_priors(const b200ba_options* o, const b200ba_covariance_options* c,
+                                                    const b200ba_problem* p, const b200ba_position_priors* priors,
+                                                    b200ba_covariance_t* out);
 /* Each getter returns the block's tangent size and writes size x size doubles (row-major), or returns 0 when the block is
  * not variable or was not estimated in this mode (the reference's nullopt). */
 int b200ba_covariance_point(b200ba_covariance_t h, int64_t point, double out[9]);
