@@ -242,6 +242,15 @@ __global__ void pm_init_kernel(const PmParams P, float* sel_prev) {
 // NCC of one (hypothesis, source image) pair by an 8-lane group
 // (PhotoConsistencyCostComputer::Compute, patch_match_cuda.cu:489-593)
 // ------------------------------------------------------------------------------------------------
+// Lane `sub` adds taps sub, sub + 8, ... in ascending order.  The loop is a software pipeline of depth D: the quad words
+// of the lane's next D - 1 taps are in flight while a tap is blended, so a warp waits on one gather latency per D taps
+// instead of one per tap.  The look-ahead index is clamped to the lane's last tap (the extra loads of the last
+// iterations re-read that word and are dropped); a lane without taps fetches slot `sub` of the padded patch, whose
+// offsets are finite, and adds nothing.  Depth and unroll per caller, by C2 run time on an H100 80GB HBM3 at 700 W
+// (DESIGN.md §2 has the grid): the pixel pass <3, 3> (P 12.65 ms per sweep against 13.43 with the loop it replaced;
+// every U = 1 point and D = 4 lost, as did 7 and 6 resident CTAs); the serial pass and the initial cost <1, 5>, where
+// ptxas already overlaps the loads of the unrolled copies (S at D = 2 or 3 took 13.4-17.2 ms per sweep against 12.2).
+template <int D, int UNROLL>
 __device__ __forceinline__ float pm_ncc_group(const float4* __restrict__ patch, int ntaps, const float* __restrict__ pose,
                                               const float iK[4], const uint32_t* __restrict__ quads, int pitch, int W,
                                               int H, float rowf, float colf, float d, float n0, float n1, float n2,
@@ -256,22 +265,35 @@ __device__ __forceinline__ float pm_ncc_group(const float4* __restrict__ patch, 
   const float cx = fmaf(Hm[0], colf, fmaf(Hm[1], rowf, Hm[2]));
   const float cy = fmaf(Hm[3], colf, fmaf(Hm[4], rowf, Hm[5]));
   const float cz = fmaf(Hm[6], colf, fmaf(Hm[7], rowf, Hm[8]));
-  auto tap = [&](int t) {
-    const float4 tp = patch[t];   // {w, w * ref, dx, dy}
-    const float zx = fmaf(Hm[0], tp.z, fmaf(Hm[1], tp.w, cx));
-    const float zy = fmaf(Hm[3], tp.z, fmaf(Hm[4], tp.w, cy));
-    const float zz = fmaf(Hm[6], tp.z, fmaf(Hm[7], tp.w, cz));
+  auto fetch = [&](int t) {
+    const float2 off = reinterpret_cast<const float2*>(&patch[t])[1];   // {dx, dy} of {w, w * ref, dx, dy}
+    const float zx = fmaf(Hm[0], off.x, fmaf(Hm[1], off.y, cx));
+    const float zy = fmaf(Hm[3], off.x, fmaf(Hm[4], off.y, cy));
+    const float zz = fmaf(Hm[6], off.x, fmaf(Hm[7], off.y, cz));
     const float inv_z = pm_rcp_clamped(zz);
-    const float color = pm_sample_quad(quads0, pitch, hi_x, hi_y, inv_z * zx, inv_z * zy);
-    const float ws = tp.x * color;
+    return pm_quad_fetch(quads0, pitch, hi_x, hi_y, inv_z * zx, inv_z * zy);
+  };
+  auto consume = [&](int t, const PmQuadTap& q) {
+    const float color = pm_quad_blend(q);
+    const float2 wr = reinterpret_cast<const float2*>(&patch[t])[0];    // {w, w * ref}
+    const float ws = wr.x * color;
     s1 += ws;
     s2 = fmaf(ws, color, s2);
-    s3 = fmaf(tp.y, color, s3);
+    s3 = fmaf(wr.y, color, s3);
   };
-  const int nfull = ntaps >> 3;  // warp-uniform trip count; the ragged tail is one predicated tap
-#pragma unroll 5
-  for (int j = 0; j < nfull; ++j) tap(sub + 8 * j);
-  if (sub < (ntaps & 7)) tap(sub + 8 * nfull);
+  const int cnt = (ntaps >> 3) + ((sub < (ntaps & 7)) ? 1 : 0);
+  const int last = sub + 8 * (cnt > 0 ? cnt - 1 : 0);
+  PmQuadTap st[D];
+#pragma unroll
+  for (int k = 0; k < D - 1; ++k) st[k] = fetch(min(sub + 8 * k, last));
+#pragma unroll UNROLL
+  for (int j = 0; j < cnt; ++j) {
+    const int t = sub + 8 * j;
+    st[D - 1] = fetch(min(t + 8 * (D - 1), last));
+    consume(t, st[0]);
+#pragma unroll
+    for (int k = 0; k < D - 1; ++k) st[k] = st[k + 1];
+  }
 #pragma unroll
   for (int o = 1; o < 8; o <<= 1) {
     s1 = s1 + __shfl_xor_sync(gmask, s1, o);
@@ -465,7 +487,7 @@ __global__ void __launch_bounds__(128) pm_initial_cost_kernel(const PmParams P) 
       const int img = base + g;
       if (img < N) {
         const PmSrcDesc sd = P.src[img];
-        const float c = pm_ncc_group(patch, P.ntaps, poses + img * PM_POSE_STRIDE, P.invK[0], P.quads + sd.quad_off,
+        const float c = pm_ncc_group<1, 5>(patch, P.ntaps, poses + img * PM_POSE_STRIDE, P.invK[0], P.quads + sd.quad_off,
                                      sd.pitch, sd.w, sd.h, (float)row, (float)col, hy.x, hy.y, hy.z, hy.w, inv_wsum,
                                      rsum, rsq, sub, gmask);
         if (sub == 0) P.cost[p * N + img] = c;
@@ -645,7 +667,7 @@ __global__ void __launch_bounds__(128, 8) pm_pixel_kernel(const PmParams P, cons
           const float hd = (hsel == 1) ? cur_d : r4.x;
           const float hn0 = (hsel == 2) ? cn0 : r4.y, hn1 = (hsel == 2) ? cn1 : r4.z, hn2 = (hsel == 2) ? cn2 : r4.w;
           const PmSrcDesc sd = P.src[img];
-          const float c = pm_ncc_group(patch, P.ntaps, poses + img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch,
+          const float c = pm_ncc_group<3, 3>(patch, P.ntaps, poses + img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch,
                                        sd.w, sd.h, rowf, colf, hd, hn0, hn1, hn2, inv_wsum, rsum, rsq, sub, gmask);
           if (sub == 0) A.tab3[(p * 3 + hsel) * N + img] = c;
         }
@@ -705,7 +727,7 @@ __global__ void __launch_bounds__(128, 8) pm_pixel_kernel(const PmParams P, cons
         const float hd = (my_k == 1) ? cur_d : r4.x;
         const float hn0 = (my_k == 2) ? cn0 : r4.y, hn1 = (my_k == 2) ? cn1 : r4.z, hn2 = (my_k == 2) ? cn2 : r4.w;
         const PmSrcDesc sd = P.src[my_img];
-        c = pm_ncc_group(patch, P.ntaps, poses + my_img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch, sd.w, sd.h,
+        c = pm_ncc_group<3, 3>(patch, P.ntaps, poses + my_img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch, sd.w, sd.h,
                          rowf, colf, hd, hn0, hn1, hn2, inv_wsum, rsum, rsq, sub, gmask);
         if (sub == 0) A.tab3[(p * 3 + my_k) * N + my_img] = c;
       }
@@ -856,7 +878,7 @@ __global__ void __launch_bounds__(32 * WPC, 16 / WPC) pm_serial_kernel(const PmP
       const float hd = hyp1[0], hn0 = hyp1[1], hn1 = hyp1[2], hn2 = hyp1[3];
       for (int img = warp * 4 + g; img < N; img += 4 * WPC) {
         const PmSrcDesc sd = P.src[img];
-        const float c = pm_ncc_group(patch, P.ntaps, poses + img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch,
+        const float c = pm_ncc_group<1, 5>(patch, P.ntaps, poses + img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch,
                                      sd.w, sd.h, rowf, colf, hd, hn0, hn1, hn2, inv_wsum, rsum, rsq, sub, gmask);
         if (sub == 0) tab1[img] = c;
       }
@@ -885,7 +907,7 @@ __global__ void __launch_bounds__(32 * WPC, 16 / WPC) pm_serial_kernel(const PmP
           float c = 0.0f;
           if (my_img >= 0) {
             const PmSrcDesc sd = P.src[my_img];
-            c = pm_ncc_group(patch, P.ntaps, poses + my_img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch, sd.w, sd.h,
+            c = pm_ncc_group<1, 5>(patch, P.ntaps, poses + my_img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch, sd.w, sd.h,
                              rowf, colf, hd, hn0, hn1, hn2, inv_wsum, rsum, rsq, sub, gmask);
           }
 #pragma unroll
