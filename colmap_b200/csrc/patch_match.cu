@@ -1048,8 +1048,7 @@ __global__ void pm_rcp_check_kernel(unsigned long long* mismatches) {
   unsigned long long bad = 0;
   for (unsigned long long b = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; b < (1ull << 32); b += stride) {
     const float z = __uint_as_float((unsigned)b);
-    const float zc = fminf(fmaxf(z, 1e-30f), 1e30f);
-    const float want = 1.0f / zc;
+    const float want = 1.0f / pm_clamp_z(z);
     const float got = pm_rcp_clamped(z);
     if (__float_as_uint(want) != __float_as_uint(got)) ++bad;
   }
@@ -1450,6 +1449,7 @@ int b200pm_run(b200pm_handle c) {
   const float total_steps = (float)(iters * 4);
   int t = 0;
   const int max_sweeps = getenv("B200PM_MAX_SWEEPS") ? atoi(getenv("B200PM_MAX_SWEEPS")) : -1;
+  c->final_sel = 1;   // until a sweep runs, the selection probability is the 0.5 that pm_init_kernel wrote to sel[1]
   for (int iter = 0; iter < iters; ++iter) {
     for (int sweep = 0; sweep < 4; ++sweep, ++t) {
       if (max_sweeps >= 0 && t >= max_sweeps) break;

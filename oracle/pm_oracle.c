@@ -38,8 +38,11 @@
  * interpolation on raw 8-bit values instead of the 9-bit-weight texture unit;
  * (3) the NCC sums are accumulated in 8 interleaved partial sums joined by a
  * fixed tree; (4) pose matrices are composed in double and rounded once;
- * (5) the per-tap projective depth is clamped to [1e-30, 1e30] before the
- * reciprocal (only matters for points behind the source camera).
+ * (5) the magnitude of the per-tap projective depth is clamped to [1e-30, 1e30]
+ * before the reciprocal, its sign kept; z = 0 and NaN sample the zero border
+ * (where the reference divides by zero).  tests/pm_fp64.py restates the
+ * reference in float64 without these deviations; tests/test_pm_fp64_cpu.py
+ * holds this file to it within fp32 error bounds.
  *
  * Build: gcc -O2 -ffp-contract=off -mfma -fopenmp -shared -fPIC (see Makefile).
  */
@@ -427,11 +430,14 @@ static float ncc_cost(const pm_state* st, const pm_patch* pt, int row, int col, 
     const float zx = fmaf(H[0], dx, fmaf(H[1], dy, cx));
     const float zy = fmaf(H[3], dx, fmaf(H[4], dy, cy));
     const float zz = fmaf(H[6], dx, fmaf(H[7], dy, cz));
-    /* points at or behind the source camera plane sample the border: z is clamped to [1e-30, 1e30]
-     * (keeps the reciprocal in the range where the GPU's MUFU.RCP + one Newton step is correctly rounded) */
-    float zc = (zz > 1e-30f) ? zz : 1e-30f;
-    zc = (zc < 1e30f) ? zc : 1e30f;
-    const float inv_z = 1.0f / zc;
+    /* |z| is clamped to [1e-30, 1e30] with its sign kept (keeps the reciprocal in the range where the GPU's
+     * MUFU.RCP + one Newton step is correctly rounded).  A point behind the source camera samples its mirror
+     * image through the camera centre, as the reference's 1 / z does (:526-535); z < 0 decides the sign, so
+     * -0 and NaN give +1e-30, which samples the zero border (pm_device.cuh:pm_clamp_z states the same rule). */
+    float za = (zz < 0.0f) ? -zz : zz;
+    za = (za > 1e-30f) ? za : 1e-30f;
+    za = (za < 1e30f) ? za : 1e30f;
+    const float inv_z = 1.0f / ((zz < 0.0f) ? -za : za);
     const float color = sample_src(st, image_idx, inv_z * zx, inv_z * zy);
     const float ws = pt->w[t] * color;
     const int q = t & 7;

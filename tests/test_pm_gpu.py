@@ -43,7 +43,7 @@ def _assert_bit_exact(got, ref, keys=("depth", "normal", "sel_prob")):
 
 
 def test_fast_reciprocal_is_ieee_over_all_floats():
-    """The per-tap reciprocal (MUFU.RCP + one Newton step after clamping to [1e-30, 1e30]) must equal the
+    """The per-tap reciprocal (MUFU.RCP + one Newton step after clamping |z| to [1e-30, 1e30], sign kept) must equal the
     correctly rounded division the oracle uses, for every one of the 2^32 float bit patterns."""
     import ctypes
     from colmap_b200 import load_library
