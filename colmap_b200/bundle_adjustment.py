@@ -137,6 +137,7 @@ class Camera:
     camera_id: int
     model_id: int
     params: np.ndarray           # float64
+    has_prior_focal_length: bool = False
 
 
 @dataclass

@@ -516,3 +516,24 @@ def synthesize_noise(rec, pose_priors=None, point2D_stddev=0.0, point3D_stddev=0
             pp.position_covariance = prior_position_stddev ** 2 * np.eye(3)
     return rec
 
+
+
+def synthesize_global_positioning(num_frames, num_points, num_observations, seed=0, ray_stddev=5e-3):
+    """A flat global-positioning problem (FlatGlobalPositioning): frame centres on a sphere of radius 5 around points in
+    the unit cube, num_observations // num_points observations per point in distinct frames, unit rays with Gaussian
+    noise of ray_stddev, the reference's random initial centres and points (100 * U(-1, 1)), unit scales and the 0.5
+    loss weight of cameras without a prior focal length."""
+    from .global_positioning import FlatGlobalPositioning
+    rng = np.random.default_rng(seed)
+    C = rng.normal(size=(num_frames, 3))
+    C *= 5 / np.linalg.norm(C, axis=1, keepdims=True)
+    X = rng.uniform(-1, 1, (num_points, 3))
+    k = num_observations // num_points
+    obs_point = np.repeat(np.arange(num_points), k)
+    obs_frame = (rng.integers(0, num_frames, num_points)[:, None] + np.arange(k)[None, :] * max(1, num_frames // k)).reshape(-1) % num_frames
+    d = X[obs_point] - C[obs_frame]
+    d /= np.linalg.norm(d, axis=1, keepdims=True)
+    d += rng.normal(0, ray_stddev, d.shape)
+    return FlatGlobalPositioning(frame_centers=100 * rng.uniform(-1, 1, (num_frames, 3)),
+                                 points=100 * rng.uniform(-1, 1, (num_points, 3)), obs_frame=obs_frame, obs_point=obs_point,
+                                 obs_ray=d, obs_scale=np.ones(len(obs_point)), obs_loss_weight=np.full(len(obs_point), 0.5))
