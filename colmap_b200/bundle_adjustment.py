@@ -184,6 +184,31 @@ class Reconstruction:
     points3D: Dict[int, Point3D] = field(default_factory=dict)
     rigs: Dict[int, Rig] = field(default_factory=dict)       # empty = trivial frames throughout
     frames: Dict[int, Frame] = field(default_factory=dict)
+    reg_frame_ids: List[int] = field(default_factory=list)   # registered frames, in registration order
+
+    def RegisterFrame(self, frame_id):
+        """Reconstruction::RegisterFrame: a frame with a pose joins the registered set (once)."""
+        if frame_id not in self.reg_frame_ids:
+            self.reg_frame_ids.append(frame_id)
+
+    def DeRegisterFrame(self, frame_id):
+        """Reconstruction::DeRegisterFrame: leaves the registered set, its images' observations are deleted and its pose
+        is reset.  A frame that is not registered is ignored."""
+        if frame_id not in self.reg_frame_ids:
+            return
+        self.reg_frame_ids.remove(frame_id)
+        for image_id, im in self.images.items():
+            if im.frame_id != frame_id:
+                continue
+            for k, p2 in enumerate(im.points2D):
+                if p2.point3D_id in self.points3D:
+                    pt = self.points3D[p2.point3D_id]
+                    pt.track = [t for t in pt.track if t != (image_id, k)]
+                p2.point3D_id = -1
+        self.frames[frame_id].rig_from_world = None
+
+    def RegFrameIds(self) -> List[int]:
+        return list(self.reg_frame_ids)
 
     def IsRefInFrame(self, image_id) -> bool:
         """Image::IsRefInFrame: the image's camera is the reference sensor of its frame's rig."""
@@ -1152,12 +1177,16 @@ class PosePrior:
     position: np.ndarray = field(default_factory=lambda: np.full(3, np.nan))
     position_covariance: np.ndarray = field(default_factory=lambda: np.full((3, 3), np.nan))
     sensor_type: str = "CAMERA"
+    gravity: np.ndarray = field(default_factory=lambda: np.full(3, np.nan))   # unit gravity direction in the camera frame
 
     def HasPosition(self) -> bool:
         return bool(np.all(np.isfinite(self.position)))
 
     def HasPositionCov(self) -> bool:
         return bool(np.all(np.isfinite(self.position_covariance)))
+
+    def HasGravity(self) -> bool:
+        return bool(np.all(np.isfinite(self.gravity)))
 
 
 @dataclass

@@ -5,7 +5,8 @@
 // tensor cores (mma.sync.aligned.m16n8k4 .f64, DMMA), four warps of 32 x 32.  The six operations differ only in where
 // the two operands come from and where the result goes (the MODE template argument).  The diagonal tiles are factorised
 // and inverted by one CTA each in shared memory (ba_tile_potrf_kernel); the panel solve then multiplies by that inverse
-// on the tensor cores, as does TRTRI.
+// on the tensor cores, as does TRTRI.  The triangular solves with the factor (ba_dense_potrs) run one 64-wide tile per
+// launch on those inverted diagonal tiles.
 #include "ba_dense_f64.h"
 
 #include <math.h>
@@ -217,5 +218,67 @@ cudaError_t ba_dense_potri(double* A, int N, const double* dinv, double* panel, 
     if (i) ba_tile_kernel<TM_LAUUM><<<i, TT, 0, st>>>(a);
     ba_tile_kernel<TM_LAUUM_D><<<1, TT, 0, st>>>(a);
   }
+  return cudaGetLastError();
+}
+
+// L L^T X = B with L from ba_dense_potrf, one 64-wide tile per launch and every launch spread over the GPU; blockIdx.y
+// is the right-hand side, and every right-hand side sees the same arithmetic in the same order.  Forward, tile k:
+// y_k = Linv_kk b_k, then b_r -= L_rk y_k for every row below the tile (one thread per row, coalesced down the
+// columns).  Backward, tile k (last first): x_k = Linv_kk^T u_k, then u_c -= L_kc^T x_k for every column left of the
+// tile (one warp per column, the tile's 64 entries of a column are contiguous).  Every CTA recomputes the tile's
+// 64-vector from the tile's inputs, which no launch writes, and CTA 0 stores it.
+#define TB 256
+__global__ void __launch_bounds__(TB) ba_trsv_fwd(const double* A, const double* dinv, int N, int k, double* B, double* Y,
+                                                  const BaDenseFlag* flag) {
+  if (flag->bad) return;
+  __shared__ double t[T], yk[T];
+  const int tid = threadIdx.x;
+  double* b = B + (long long)blockIdx.y * N;
+  double* y = Y + (long long)blockIdx.y * N;
+  const double* X = dinv + (long long)k * T * T;
+  if (tid < T) t[tid] = b[k * T + tid];
+  __syncthreads();
+  if (tid < T) { double s = 0; for (int c = 0; c <= tid; ++c) s += X[c * T + tid] * t[c]; yk[tid] = s; }
+  __syncthreads();
+  if (blockIdx.x == 0 && tid < T) y[k * T + tid] = yk[tid];
+  const int r = (k + 1) * T + blockIdx.x * TB + tid;
+  if (r >= N) return;
+  const double* col = A + (long long)k * T * N + r;
+  double s = 0;
+  for (int c = 0; c < T; ++c) s += col[(long long)c * N] * yk[c];
+  b[r] -= s;
+}
+
+__global__ void __launch_bounds__(TB) ba_trsv_bwd(const double* A, const double* dinv, int N, int k, double* U, double* B,
+                                                  const BaDenseFlag* flag) {
+  if (flag->bad) return;
+  __shared__ double t[T], xk[T];
+  const int tid = threadIdx.x;
+  double* u = U + (long long)blockIdx.y * N;
+  double* x = B + (long long)blockIdx.y * N;
+  const double* X = dinv + (long long)k * T * T;
+  if (tid < T) t[tid] = u[k * T + tid];
+  __syncthreads();
+  if (tid < T) { double s = 0; for (int r = tid; r < T; ++r) s += X[tid * T + r] * t[r]; xk[tid] = s; }
+  __syncthreads();
+  if (blockIdx.x == 0 && tid < T) x[k * T + tid] = xk[tid];
+  const int warp = tid / 32, lane = tid % 32;
+  const int c = blockIdx.x * (TB / 32) + warp;
+  if (c >= k * T) return;
+  const double* L = A + (long long)c * N + k * T;
+  double s = L[lane] * xk[lane] + L[lane + 32] * xk[lane + 32];
+  for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) u[c] -= s;
+}
+
+static inline unsigned ba_blocks(long long n, int t) { return (unsigned)(n > 0 ? (n + t - 1) / t : 1); }
+
+cudaError_t ba_dense_potrs(const double* A, int N, const double* dinv, int nrhs, double* B, double* W, const BaDenseFlag* flag,
+                           cudaStream_t st) {
+  const int nt = N / T;
+  for (int k = 0; k < nt; ++k)
+    ba_trsv_fwd<<<dim3(ba_blocks(N - (long long)(k + 1) * T, TB), nrhs), TB, 0, st>>>(A, dinv, N, k, B, W, flag);
+  for (int k = nt - 1; k >= 0; --k)
+    ba_trsv_bwd<<<dim3(ba_blocks((long long)k * T, TB / 32), nrhs), TB, 0, st>>>(A, dinv, N, k, W, B, flag);
   return cudaGetLastError();
 }

@@ -1,5 +1,6 @@
 // ba_dense_f64.h — tiled fp64 Cholesky and SPD inverse on the H100's fp64 tensor cores (mma.sync m16n8k4 .f64).
-// Used by the bundle-adjustment covariance estimate (b200ba_estimate_covariance) on the reduced camera-side matrix.
+// Used by the bundle-adjustment covariance estimate (b200ba_estimate_covariance) on the reduced camera-side matrix, and
+// by the global positioning and rotation averaging solves.
 //
 // Layout: an N x N column-major matrix, N a multiple of BA_TILE; element (i, j), i >= j, lives at A[j * N + i] (the
 // layout of the solve's dense reduced matrix).  Only the lower triangle is input and output.  Outside the 64 x 64
@@ -27,3 +28,8 @@ cudaError_t ba_dense_potrf(double* A, int N, int n_test0, int n_check, double pi
                            cudaStream_t st);
 // A (holding L from ba_dense_potrf) <- (L L^T)^-1 = L^-T L^-1, lower triangle: TRTRI then LAUUM.  panel: [N * BA_TILE] scratch.
 cudaError_t ba_dense_potri(double* A, int N, const double* dinv, double* panel, const BaDenseFlag* flag, cudaStream_t st);
+// Solve L L^T X = B for nrhs right-hand sides with L and dinv from ba_dense_potrf.  B: [nrhs * N] column-major (ld N),
+// the right-hand sides in, the solutions out; W: [nrhs * N] scratch.  Each right-hand side sees the same arithmetic in
+// the same order whatever nrhs is.  Returns at once on every launch when flag->bad is set.
+cudaError_t ba_dense_potrs(const double* A, int N, const double* dinv, int nrhs, double* B, double* W, const BaDenseFlag* flag,
+                           cudaStream_t st);

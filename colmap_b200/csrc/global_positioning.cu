@@ -6,7 +6,7 @@
 //   2. per point: eliminate the 3x3 point block (observations are sorted by point),
 //   3. the reduced matrix over frame centres and camera-in-rig positions (3 columns per block) is built densely, one
 //      thread per row and no atomics, so that repeated solves are bit-identical; the LM diagonal is added,
-//   4. ba_dense_potrf factors it, forward / backward solves one tile per launch on the inverted diagonal tiles give the step,
+//   4. ba_dense_potrf factors it, ba_dense_potrs (forward / backward solves one tile per launch) gives the step,
 //   5. back-substitution to the points, then to the scales.
 // Trust-region rules (Jacobi scaling from the first Jacobian, LM diagonal clamp, radius update, tolerances) are those of
 // oracle/ba_oracle.c; the scale bound is enforced as ceres::ParameterBlock::Plus does, by clamping the candidate, while
@@ -423,52 +423,6 @@ __global__ void k_pad_identity(double* A, int n, int Npad) {
   if (i < Npad) A[(int64_t)i * Npad + i] = 1.0;
 }
 
-// L L^T x = b with L from ba_dense_potrf (lower, column-major) and dinv its inverted diagonal tiles, one 64-wide tile
-// per launch and every launch spread over the GPU.  Forward, tile k: y_k = Linv_kk b_k, then b_r -= L_rk y_k for every
-// row below the tile (one thread per row, coalesced down the columns).  Backward, tile k (last first):
-// x_k = Linv_kk^T u_k, then u_c -= L_kc^T x_k for every column left of the tile (one warp per column, the tile's 64
-// entries of a column are contiguous).  Every CTA recomputes the tile's 64-vector from the tile's inputs, which no launch
-// writes, and CTA 0 stores it.
-#define GP_TB 256
-__global__ void __launch_bounds__(GP_TB) k_trsv_fwd(const double* A, const double* dinv, int Npad, int k, double* b, double* y,
-                                                    const BaDenseFlag* flag) {
-  if (flag->bad) return;
-  __shared__ double t[BA_TILE], yk[BA_TILE];
-  const int tid = threadIdx.x;
-  const double* X = dinv + (int64_t)k * BA_TILE * BA_TILE;
-  if (tid < BA_TILE) t[tid] = b[k * BA_TILE + tid];
-  __syncthreads();
-  if (tid < BA_TILE) { double s = 0; for (int c = 0; c <= tid; ++c) s += X[c * BA_TILE + tid] * t[c]; yk[tid] = s; }
-  __syncthreads();
-  if (blockIdx.x == 0 && tid < BA_TILE) y[k * BA_TILE + tid] = yk[tid];
-  const int r = (k + 1) * BA_TILE + blockIdx.x * GP_TB + tid;
-  if (r >= Npad) return;
-  const double* col = A + (int64_t)k * BA_TILE * Npad + r;
-  double s = 0;
-  for (int c = 0; c < BA_TILE; ++c) s += col[(int64_t)c * Npad] * yk[c];
-  b[r] -= s;
-}
-
-__global__ void __launch_bounds__(GP_TB) k_trsv_bwd(const double* A, const double* dinv, int Npad, int k, double* u, double* x,
-                                                    const BaDenseFlag* flag) {
-  if (flag->bad) return;
-  __shared__ double t[BA_TILE], xk[BA_TILE];
-  const int tid = threadIdx.x;
-  const double* X = dinv + (int64_t)k * BA_TILE * BA_TILE;
-  if (tid < BA_TILE) t[tid] = u[k * BA_TILE + tid];
-  __syncthreads();
-  if (tid < BA_TILE) { double s = 0; for (int r = tid; r < BA_TILE; ++r) s += X[tid * BA_TILE + r] * t[r]; xk[tid] = s; }
-  __syncthreads();
-  if (blockIdx.x == 0 && tid < BA_TILE) x[k * BA_TILE + tid] = xk[tid];
-  const int warp = tid / 32, lane = tid % 32;
-  const int c = blockIdx.x * (GP_TB / 32) + warp;
-  if (c >= k * BA_TILE) return;
-  const double* L = A + (int64_t)c * Npad + k * BA_TILE;
-  double s = L[lane] * xk[lane] + L[lane + 32] * xk[lane + 32];
-  for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  if (lane == 0) u[c] -= s;
-}
-
 // back-substitution to the points: dX = H^-1 (-g_p - sum E dC)
 __global__ void k_back_points(GpDev g) {
   const int64_t vp = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -746,12 +700,8 @@ extern "C" int b200gp_solve(const b200gp_options* o, b200gp_problem* p, b200gp_s
           if (Npad > n) k_pad_identity<<<gp_blocks(Npad - n, 64), 64>>>(g.A, n, Npad);
           GP_CUDA(cudaMemcpy(g.dC, g.rhs, sizeof(double) * Npad, cudaMemcpyDeviceToDevice));
           GP_CUDA(ba_dense_potrf(g.A, Npad, n, n, 0.0, g.dinv, g.flag, 0));
-          // forward: b in dC, y into rhs; backward: u = y in rhs, x into dC
-          const int nt = Npad / BA_TILE;
-          for (int k = 0; k < nt; ++k)
-            k_trsv_fwd<<<gp_blocks(Npad - (k + 1) * BA_TILE, GP_TB), GP_TB>>>(g.A, g.dinv, Npad, k, g.dC, g.rhs, g.flag);
-          for (int k = nt - 1; k >= 0; --k)
-            k_trsv_bwd<<<gp_blocks((int64_t)k * BA_TILE, GP_TB / 32), GP_TB>>>(g.A, g.dinv, Npad, k, g.rhs, g.dC, g.flag);
+          // b in dC, the solution back into dC; rhs is the scratch
+          GP_CUDA(ba_dense_potrs(g.A, Npad, g.dinv, 1, g.dC, g.rhs, g.flag, 0));
         }
         if (nvp) k_back_points<<<gp_blocks(nvp, 128), 128>>>(g);
         k_back_obs<<<gp_blocks(N, 256), 256>>>(g, d_pvar);

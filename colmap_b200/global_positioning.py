@@ -11,12 +11,12 @@ then camera-in-rig positions) from numpy's ``default_rng(random_seed)``.  That s
 """
 import ctypes
 from dataclasses import dataclass, field
-from typing import List, Optional, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 
 from ._lib import load_library
-from .bundle_adjustment import CONVERGENCE, FAILURE, NO_CONVERGENCE, Reconstruction, _quat_to_R
+from .bundle_adjustment import CONVERGENCE, FAILURE, NO_CONVERGENCE, Reconstruction, _quat_to_R, _rigid_inverse
 
 SCALE_LOWER_BOUND = 1e-5
 MAX_REDUCED_DIM = 32768
@@ -186,12 +186,95 @@ def cam_ray_from_img(model_id: int, params, xy) -> Optional[np.ndarray]:
 
 
 @dataclass
+class PoseGraphEdge:
+    """PoseGraph::Edge: the relative pose cam2_from_cam1 (7: qx qy qz qw tx ty tz), the inlier match count and the
+    valid flag."""
+    cam2_from_cam1: np.ndarray = field(default_factory=lambda: np.array([0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0]))
+    num_matches: int = 0
+    valid: bool = True
+
+
+@dataclass
 class PoseGraph:
-    """The part of PoseGraph the positioner reads: its valid edges as (image_id1, image_id2) pairs."""
+    """PoseGraph (scene/pose_graph.h): edges between images keyed by pair (image_id1 < image_id2).  ``edges`` lists the
+    pairs; ``edge_data`` holds an edge's relative pose, match count and valid flag (an edge without data is valid, with
+    the identity pose and no matches), so PoseGraph(edges=[...]) still builds the graph the global positioner reads."""
     edges: List[Tuple[int, int]] = field(default_factory=list)
+    edge_data: Dict[Tuple[int, int], PoseGraphEdge] = field(default_factory=dict)
+
+    @staticmethod
+    def _key(i1, i2):
+        return (i1, i2) if i1 < i2 else (i2, i1)
+
+    def AddEdge(self, image_id1, image_id2, edge: PoseGraphEdge):
+        """Stores the edge under its pair; given as (larger, smaller) id, cam2_from_cam1 is inverted."""
+        if image_id1 > image_id2:
+            edge = PoseGraphEdge(_rigid_inverse(edge.cam2_from_cam1), edge.num_matches, edge.valid)
+            image_id1, image_id2 = image_id2, image_id1
+        if (image_id1, image_id2) not in self.edge_data and (image_id1, image_id2) not in self.edges:
+            self.edges.append((image_id1, image_id2))
+        self.edge_data[(image_id1, image_id2)] = edge
+
+    def DeleteEdge(self, image_id1, image_id2):
+        k = self._key(image_id1, image_id2)
+        self.edges = [e for e in self.edges if self._key(*e) != k]
+        self.edge_data.pop(k, None)
+
+    def Edges(self) -> Dict[Tuple[int, int], PoseGraphEdge]:
+        """Every edge by pair, in pair order."""
+        return {k: self.EdgeData(*k) for k in sorted(self._key(*e) for e in self.edges)}
+
+    def EdgeData(self, image_id1, image_id2) -> PoseGraphEdge:
+        k = self._key(image_id1, image_id2)
+        if k not in self.edge_data:
+            self.edge_data[k] = PoseGraphEdge()
+        return self.edge_data[k]
+
+    def GetEdge(self, image_id1, image_id2) -> PoseGraphEdge:
+        """The edge from image_id1 to image_id2 (inverted when stored the other way)."""
+        e = self.EdgeData(image_id1, image_id2)
+        return e if image_id1 < image_id2 else PoseGraphEdge(_rigid_inverse(e.cam2_from_cam1), e.num_matches, e.valid)
+
+    def NumEdges(self):
+        return len(self.edges)
 
     def ValidEdges(self):
-        return list(self.edges)
+        """The valid edges as (image_id1, image_id2) pairs, in insertion order."""
+        return [e for e in self.edges if self.EdgeData(*e).valid]
+
+    def SetInvalidEdge(self, image_id1, image_id2):
+        self.EdgeData(image_id1, image_id2).valid = False
+
+    def InvalidatePairsOutsideActiveImageIds(self, active_image_ids):
+        for e in self.edges:
+            if e[0] not in active_image_ids or e[1] not in active_image_ids:
+                self.SetInvalidEdge(*e)
+
+    def ComputeLargestConnectedFrameComponent(self, rec, filter_unregistered=False):
+        """The frames of the largest connected component of the valid edges (images must have frames); ties go to the
+        component with the smallest frame id."""
+        parent = {}
+
+        def find(a):
+            while parent[a] != a:
+                parent[a] = parent[parent[a]]
+                a = parent[a]
+            return a
+        for i1, i2 in self.ValidEdges():
+            f1, f2 = rec.images[i1].frame_id, rec.images[i2].frame_id
+            if filter_unregistered and (rec.frames[f1].rig_from_world is None or rec.frames[f2].rig_from_world is None):
+                continue
+            parent.setdefault(f1, f1)
+            parent.setdefault(f2, f2)
+            a, b = find(f1), find(f2)
+            if a != b:
+                parent[max(a, b)] = min(a, b)
+        comps = {}
+        for f in parent:
+            comps.setdefault(find(f), set()).add(f)
+        if not comps:
+            return set()
+        return max(comps.values(), key=lambda c: (len(c), -min(c)))
 
 
 class GlobalPositioner:

@@ -537,3 +537,158 @@ def synthesize_global_positioning(num_frames, num_points, num_observations, seed
     return FlatGlobalPositioning(frame_centers=100 * rng.uniform(-1, 1, (num_frames, 3)),
                                  points=100 * rng.uniform(-1, 1, (num_points, 3)), obs_frame=obs_frame, obs_point=obs_point,
                                  obs_ray=d, obs_scale=np.ones(len(obs_point)), obs_loss_weight=np.full(len(obs_point), 0.5))
+
+
+def _random_rotations(rng, n):
+    q = rng.normal(size=(n, 4))
+    q /= np.linalg.norm(q, axis=1, keepdims=True)
+    x, y, z, w = q.T
+    return np.stack([1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
+                     2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
+                     2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)], 1).reshape(n, 3, 3)
+
+
+def _exp_so3(w):
+    w = np.asarray(w, np.float64).reshape(-1, 3)
+    th = np.linalg.norm(w, axis=1)
+    a = w / np.where(th > 0, th, 1.0)[:, None]
+    K = np.zeros((len(w), 3, 3))
+    K[:, 0, 1], K[:, 0, 2], K[:, 1, 2] = -a[:, 2], a[:, 1], -a[:, 0]
+    K[:, 1, 0], K[:, 2, 0], K[:, 2, 1] = a[:, 2], -a[:, 1], a[:, 0]
+    s, c = np.sin(th)[:, None, None], np.cos(th)[:, None, None]
+    return c * np.eye(3) + (1 - c) * a[:, :, None] * a[:, None, :] + s * K
+
+
+def _log_so3(R):
+    R = np.asarray(R).reshape(-1, 3, 3)
+    c = np.clip((np.trace(R, axis1=1, axis2=2) - 1) / 2, -1, 1)
+    th = np.arccos(c)
+    v = np.stack([R[:, 2, 1] - R[:, 1, 2], R[:, 0, 2] - R[:, 2, 0], R[:, 1, 0] - R[:, 0, 1]], 1)
+    s = np.sin(th)
+    f = np.where(s > 1e-12, th / np.where(s > 1e-12, 2 * s, 1.0), 0.5)
+    return f[:, None] * v
+
+
+def synthesize_rotation_averaging(num_frames, edges_per_frame=20, noise_deg=1.0, outlier_ratio=0.1, seed=0,
+                                  init_noise_deg=5.0, gravity_fraction=0.0, num_cameras=0, reweighting=False,
+                                  banded=False):
+    """A flat rotation-averaging problem (FlatRotationAveraging) and its ground-truth rotations.
+
+    Frames get uniformly random rotations (a gravity-aligned 1-DOF frame a rotation about y); about
+    num_frames * edges_per_frame / 2 pairs join them: a chain through all frames plus random pairs, or, with banded,
+    each frame with its next edges_per_frame / 2 frames.  Relative rotations carry Gaussian angle-axis noise of
+    noise_deg, and a fraction outlier_ratio of them is replaced by a random rotation.  Pairs between two 1-DOF frames
+    are 1-DOF (angle and xz_error).  With num_cameras > 0, one image of some 3-DOF pairs sits in an estimated camera c
+    with a random cam_from_rig.  The initial estimate is the ground truth perturbed by init_noise_deg (y only for 1-DOF
+    frames; cameras as after the reference's rig initialisation); the gauge is the first 1-DOF frame if there is one, else frame 0, fixed at its
+    initial rotation.  Returns (flat, gt) with gt the ground-truth parameter vector."""
+    from .rotation_averaging import FlatRotationAveraging
+    rng = np.random.default_rng(seed)
+    F, C = num_frames, num_cameras
+    dof = np.where(rng.uniform(size=F) < gravity_fraction, 1, 3).astype(np.uint8)
+    Rg = _random_rotations(rng, F)
+    ang = rng.uniform(-np.pi, np.pi, F)
+    one = dof == 1
+    if one.any():
+        Rg[one] = _exp_so3(np.stack([np.zeros(one.sum()), ang[one], np.zeros(one.sum())], 1))
+    Rc = _random_rotations(rng, C) if C else np.zeros((0, 3, 3))
+    k = max(1, edges_per_frame // 2)
+    if banded:
+        pairs = [(i, j) for i in range(F) for j in range(i + 1, min(F, i + 1 + k))]
+    else:
+        pairs = {(i, i + 1) for i in range(F - 1)}
+        target = max(len(pairs), F * k)
+        while len(pairs) < target:
+            a, b = rng.integers(0, F, 2)
+            if a != b:
+                pairs.add((min(a, b), max(a, b)))
+        pairs = sorted(pairs)
+    P = len(pairs)
+    f1 = np.array([p[0] for p in pairs], np.int32).reshape(-1)
+    f2 = np.array([p[1] for p in pairs], np.int32).reshape(-1)
+    pdof = np.where(one[f1] & one[f2], 1, 3).astype(np.uint8)
+    c1 = np.full(P, -1, np.int32)
+    c2 = np.full(P, -1, np.int32)
+    if C:
+        sel = (pdof == 3) & (rng.uniform(size=P) < 0.5)
+        which = rng.integers(0, 2, P)
+        cam = rng.integers(0, C, P)
+        c1[sel & (which == 0)] = cam[sel & (which == 0)]
+        c2[sel & (which == 1)] = cam[sel & (which == 1)]
+    R1 = Rg[f1].copy()
+    R2 = Rg[f2].copy()
+    m1, m2 = c1 >= 0, c2 >= 0
+    R1[m1] = Rc[c1[m1]] @ R1[m1]
+    R2[m2] = Rc[c2[m2]] @ R2[m2]
+    R12 = R2 @ np.transpose(R1, (0, 2, 1))
+    R12 = _exp_so3(rng.normal(0, np.radians(noise_deg), (P, 3))) @ R12
+    out = rng.uniform(size=P) < outlier_ratio
+    if out.any():
+        R12[out] = _random_rotations(rng, int(out.sum()))
+    pangle = np.zeros(P)
+    pxz = np.zeros(P)
+    if (pdof == 1).any():
+        s = pdof == 1
+        pangle[s] = ang[f2[s]] - ang[f1[s]] + rng.normal(0, np.radians(noise_deg), s.sum())
+        pangle[s & out] = rng.uniform(-np.pi, np.pi, (s & out).sum())
+        pxz[s] = rng.normal(0, np.radians(noise_deg), s.sum()) ** 2
+    # parameters: ground truth and initial estimate
+    gt, x0 = [], []
+    for f in range(F):
+        if dof[f] == 1:
+            gt.append([ang[f]])
+            x0.append([ang[f] + rng.normal(0, np.radians(init_noise_deg))])
+        else:
+            w = _log_so3(Rg[f])[0]
+            gt.append(w)
+            x0.append(_log_so3(_exp_so3(rng.normal(0, np.radians(init_noise_deg), 3)) @ Rg[f])[0])
+    for c in range(C):
+        gt.append(_log_so3(Rc[c])[0])
+        x0.append(_log_so3(_exp_so3(rng.normal(0, np.radians(init_noise_deg), 3)) @ Rc[c])[0])
+    gt = np.concatenate([np.asarray(g, np.float64).reshape(-1) for g in gt])
+    x0 = np.concatenate([np.asarray(g, np.float64).reshape(-1) for g in x0])
+    gauge = int(np.argmax(one)) if one.any() else 0
+    off = np.concatenate([[0], np.cumsum(dof.astype(np.int64))[:-1]])
+    g0 = np.zeros(3)
+    if dof[gauge] == 1:
+        g0[1] = x0[off[gauge]]
+    else:
+        g0[:] = x0[off[gauge]:off[gauge] + 3]
+    cs, cf = None, None
+    if C:
+        lists = [sorted(set(f1[c1 == c].tolist()) | set(f2[c2 == c].tolist())) or [0] for c in range(C)]
+        cs = np.concatenate([[0], np.cumsum([len(x) for x in lists])]).astype(np.int32)
+        cf = np.concatenate([np.asarray(x, np.int32) for x in lists])
+    flat = FlatRotationAveraging(frame_dof=dof, rotations=x0, pair_frame1=f1, pair_frame2=f2, pair_dof=pdof, pair_R=R12,
+                                 gauge_frame=gauge, gauge_rotation=g0, num_cameras=C,
+                                 pair_cam1=c1 if C else None, pair_cam2=c2 if C else None,
+                                 pair_angle=pangle if (pdof == 1).any() else None,
+                                 pair_xz_error=pxz if (pdof == 1).any() else None,
+                                 pair_reweighting=rng.uniform(0.05, 1.0, P) if reweighting else None,
+                                 cam_frame_start=cs, cam_frames=cf)
+    return flat, gt
+
+
+def synthesize_pose_graph(rec, noise_deg=0.0, outlier_ratio=0.0, seed=0, gravity=False, max_num_matches=500):
+    """A PoseGraph over every image pair of ``rec`` (a reconstruction with frames, e.g. from
+    synthesize_rig_reconstruction) and its pose priors.  Each edge holds the true cam2_from_cam1 rotation (translation
+    left at zero) with Gaussian angle-axis noise of noise_deg, a fraction outlier_ratio of them replaced by a random
+    rotation, and a random inlier match count in [max_num_matches / 10, max_num_matches].  With gravity, every image
+    gets a PosePrior whose gravity is the world's +y axis in the camera frame.  Returns (pose_graph, pose_priors)."""
+    from .bundle_adjustment import PosePrior, _quat_to_R
+    from .global_positioning import PoseGraph, PoseGraphEdge
+    from .rotation_averaging import _R_to_quat
+    rng = np.random.default_rng(seed)
+    ids = sorted(rec.images)
+    R = {i: _quat_to_R(rec.images[i].cam_from_world[:4]) for i in ids}
+    pg = PoseGraph()
+    for a in range(len(ids)):
+        for b in range(a + 1, len(ids)):
+            i1, i2 = ids[a], ids[b]
+            R12 = _exp_so3(rng.normal(0, np.radians(noise_deg), 3))[0] @ R[i2] @ R[i1].T
+            if rng.uniform() < outlier_ratio:
+                R12 = _random_rotations(rng, 1)[0]
+            n = int(rng.integers(max_num_matches // 10, max_num_matches + 1))
+            pg.AddEdge(i1, i2, PoseGraphEdge(np.concatenate([_R_to_quat(R12), np.zeros(3)]), n))
+    priors = [PosePrior(i, gravity=R[i] @ np.array([0.0, 1.0, 0.0])) for i in ids] if gravity else []
+    return pg, priors
