@@ -4163,6 +4163,26 @@ int b200ba_test_dense_f64(double* A, int N, int n_test0, int n_check, double piv
   return flag.bad ? 1 : 0;
 }
 
+// ---- hook for the GPU test tier: the triangular solves alone ----
+// ba_dense_potrf (positivity test up to n_check) then ba_dense_potrs on the caller's device matrix A (as above), nrhs
+// device columns B (ld N, solved in place) and device scratch W (nrhs * N), on the legacy default stream.  Returns 0,
+// 1 after a failed pivot (its row and value in bad_row / bad_pivot; the solve's launches then return at once), or < 0.
+int b200ba_test_dense_potrs(double* A, int N, int n_check, int nrhs, double* B, double* W, int* bad_row, double* bad_pivot) {
+  if (!A || !B || !W || !bad_row || !bad_pivot) return ba_fail(-1, "null argument");
+  if (N <= 0 || N % BA_TILE || N > BA_COV_MAX_N) return ba_fail(-2, "N must be a positive multiple of 64 up to 32768");
+  if (nrhs <= 0 || nrhs > 65535) return ba_fail(-3, "nrhs must be in 1..65535");
+  BaPool work;
+  BaDenseFlag flag = {}, *d_flag;
+  double* dinv;
+  BA_CUDA(work.alloc(&d_flag, 1)); BA_CUDA(work.alloc(&dinv, (size_t)N * BA_TILE));
+  BA_CUDA(cudaMemsetAsync(d_flag, 0, sizeof(BaDenseFlag), 0));
+  BA_CUDA(ba_dense_potrf(A, N, n_check, n_check, 0.0, dinv, d_flag, 0));
+  BA_CUDA(ba_dense_potrs(A, N, dinv, nrhs, B, W, d_flag, 0));
+  BA_CUDA(cudaMemcpy(&flag, d_flag, sizeof(flag), cudaMemcpyDeviceToHost));
+  *bad_row = flag.row; *bad_pivot = flag.pivot;
+  return flag.bad ? 1 : 0;
+}
+
 void b200ba_covariance_options_init(b200ba_covariance_options* c) { c->params = B200BA_COV_ALL; c->damping = 1e-8; }
 
 int b200ba_estimate_covariance(const b200ba_options* o, const b200ba_covariance_options* c, const b200ba_problem* p,

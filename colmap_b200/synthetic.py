@@ -571,10 +571,13 @@ def _log_so3(R):
 
 def synthesize_rotation_averaging(num_frames, edges_per_frame=20, noise_deg=1.0, outlier_ratio=0.1, seed=0,
                                   init_noise_deg=5.0, gravity_fraction=0.0, num_cameras=0, reweighting=False,
-                                  banded=False):
+                                  banded=False, gravity_frames=None):
     """A flat rotation-averaging problem (FlatRotationAveraging) and its ground-truth rotations.
 
-    Frames get uniformly random rotations (a gravity-aligned 1-DOF frame a rotation about y); about
+    A frame is gravity-aligned (1-DOF) with probability gravity_fraction, or, when gravity_frames (a boolean mask over
+    the frames) is given, exactly where the mask is set; the random stream is the same either way, so everything else
+    stays as gravity_fraction would draw it.  Frames get uniformly random rotations (a gravity-aligned 1-DOF frame a
+    rotation about y); about
     num_frames * edges_per_frame / 2 pairs join them: a chain through all frames plus random pairs, or, with banded,
     each frame with its next edges_per_frame / 2 frames.  Relative rotations carry Gaussian angle-axis noise of
     noise_deg, and a fraction outlier_ratio of them is replaced by a random rotation.  Pairs between two 1-DOF frames
@@ -586,6 +589,11 @@ def synthesize_rotation_averaging(num_frames, edges_per_frame=20, noise_deg=1.0,
     rng = np.random.default_rng(seed)
     F, C = num_frames, num_cameras
     dof = np.where(rng.uniform(size=F) < gravity_fraction, 1, 3).astype(np.uint8)
+    if gravity_frames is not None:
+        mask = np.asarray(gravity_frames, bool)
+        if mask.shape != (F,):
+            raise ValueError(f"gravity_frames must be a boolean mask of {F} frames, not of shape {mask.shape}")
+        dof = np.where(mask, 1, 3).astype(np.uint8)
     Rg = _random_rotations(rng, F)
     ang = rng.uniform(-np.pi, np.pi, F)
     one = dof == 1

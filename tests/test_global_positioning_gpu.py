@@ -95,6 +95,24 @@ def test_large_reduced_system():
     assert s.num_successful_steps >= 5 and s.final_cost < 1e-2 * s.initial_cost
 
 
+@pytest.mark.parametrize("frames,dim", [(21, 63), (22, 66), (64, 192), (65, 195)])
+def test_reduced_system_at_tile_edges(frames, dim):
+    """Reduced sizes around the 64-row tile of the dense factorisation and triangular solves: one padding row (63),
+    three rows into the second tile (66), exactly three tiles without padding (192), one row past them (195)."""
+    f = synthesize_global_positioning(frames, 300, 2100, seed=frames)
+    s, _ = compare(f, GlobalPositionerOptions())
+    assert s.reduced_dim == dim
+
+
+def test_variable_rig_sensors_in_a_later_tile():
+    """2 rigs x 3 cameras x 30 frames: the 60 frame blocks fill rows 0-179 (tiles 0 to 2) and the 4 variable
+    camera-in-rig blocks, after the frames, rows 180-191 of tile 2, so most of each sensor's frames lie in other tiles."""
+    f = flat_of(2, 3, 30, nan_sensor=True, seed=3, points=60)
+    assert len(f.cams_in_rig) == 4
+    s, _ = compare(f, GlobalPositionerOptions())
+    assert s.reduced_dim == 192
+
+
 @pytest.mark.parametrize("rigs,cams,frames,refine", [(1, 1, 10, True), (2, 3, 5, True), (2, 3, 5, False)],
                          ids=["Nominal", "MultiCameraRig", "RefineSensorFromRigFalsePreservesRig"])
 def test_reference_scenarios(rigs, cams, frames, refine):

@@ -2,6 +2,7 @@
 reference's rotation_averaging_test.cc, the exact per-axis split of the normal matrix that the GPU factors, the host
 input checks of b200ra_solve, which refuse before any device work, and the ABI surface."""
 import ctypes
+import hashlib
 
 import numpy as np
 import pytest
@@ -216,3 +217,80 @@ def test_abi_surface():
     assert (d.max_num_l1_iterations, d.max_num_irls_iterations, d.irls_loss_parameter_sigma) == (5, 100, 5.0)
     assert lib.b200ra_solve(None, None, None) == ERR_INPUT
     assert b"null" in lib.b200ra_last_error()
+
+
+# Fingerprints of synthesize_rotation_averaging's output before it took gravity_frames: the sha256 (first 16 hex
+# digits) of the integer arrays and the gauge frame, and position-weighted sums of the float arrays and of the ground
+# truth.  Every seeded test of rotation averaging depends on the generator drawing the same problem.  The sums are held
+# to 1e-12 rather than bit for bit because numpy's sin and cos may round differently on another CPU's vector path; a
+# shifted random stream changes them at order one.
+GENERATOR_FINGERPRINTS = [
+    (dict(num_frames=40, edges_per_frame=10, seed=0), "b14fb02df765afb1",
+     [-36.70610160086049, -143.12507364371217, None, None, None, 6.836943981730275, -40.30174016915096]),
+    (dict(num_frames=40, edges_per_frame=10, seed=4, gravity_fraction=0.5, reweighting=True), "340fbce35dbf0ac0",
+     [57.509937664096704, 4.666506638549784, -137.91220028047866, 0.015874411227268525, 432.13480265498293,
+      2.042467344288341, 73.46017945934442]),
+    (dict(num_frames=40, edges_per_frame=10, seed=8, num_cameras=2), "451bd0199076fbf9",
+     [-109.47876209816344, 42.05142967599167, None, None, None, 4.799817268449409, -137.79830597548076]),
+    (dict(num_frames=300, edges_per_frame=12, seed=21, gravity_fraction=0.3, num_cameras=3), "908081079806de4e",
+     [126.31189741057753, 501.38762674331446, 22.20029283174202, 0.1992239450052575, None, 5.612510932101304,
+      59.195283003961485]),
+    (dict(num_frames=8, edges_per_frame=6, noise_deg=0.0, outlier_ratio=0.0, seed=9, banded=True), "273ec9bb555e94ac",
+     [-28.99511339041858, 102.66577459317047, None, None, None, -7.180252214228349, -24.870489115164464]),
+    (dict(num_frames=200, edges_per_frame=20, seed=5, gravity_fraction=0.3, reweighting=True, banded=True),
+     "9523d2f07442448d", [20.446003488378643, 626.184500360099, -69.31777356063616, 0.21922994939722318,
+                          4099.673593695615, -4.440329584599022, 64.85640659222202]),
+]
+_INT_FIELDS = ("frame_dof", "pair_frame1", "pair_frame2", "pair_dof", "pair_cam1", "pair_cam2", "cam_frame_start", "cam_frames")
+_FLOAT_FIELDS = ("rotations", "pair_R", "pair_angle", "pair_xz_error", "pair_reweighting", "gauge_rotation")
+
+
+def _generator_fingerprint(flat, gt):
+    h = hashlib.sha256()
+    for k in _INT_FIELDS:
+        a = getattr(flat, k)
+        h.update(b"-" if a is None else np.ascontiguousarray(a).tobytes())
+    h.update(str(flat.gauge_frame).encode())
+    sums = []
+    for a in [getattr(flat, k) for k in _FLOAT_FIELDS] + [gt]:
+        sums.append(None if a is None else float(np.dot(a.reshape(-1), 1.0 + np.arange(a.size) % 7)))
+    return h.hexdigest()[:16], sums
+
+
+def _same_problem(a, b):
+    for k in _INT_FIELDS + _FLOAT_FIELDS:
+        x, y = getattr(a, k), getattr(b, k)
+        assert (x is None) == (y is None), k
+        if x is not None:
+            assert x.dtype == y.dtype and np.array_equal(x.view(np.uint8), y.view(np.uint8)), k
+    assert (a.gauge_frame, a.num_cameras) == (b.gauge_frame, b.num_cameras)
+
+
+@pytest.mark.parametrize("case", range(len(GENERATOR_FINGERPRINTS)))
+def test_generator_unchanged_by_gravity_frames(case):
+    """The default draws the problem it drew before gravity_frames existed, and passing the mask the default would
+    draw reproduces the default output bit for bit (the argument does not shift the random stream)."""
+    kw, digest, sums = GENERATOR_FINGERPRINTS[case]
+    flat, gt = synthesize_rotation_averaging(**kw)
+    d, s = _generator_fingerprint(flat, gt)
+    assert d == digest
+    assert [x is None for x in s] == [x is None for x in sums]
+    np.testing.assert_allclose([x for x in s if x is not None], [x for x in sums if x is not None], rtol=1e-12, atol=0)
+    flat2, gt2 = synthesize_rotation_averaging(**kw, gravity_frames=flat.frame_dof == 1)
+    _same_problem(flat, flat2)
+    assert np.array_equal(gt.view(np.uint64), gt2.view(np.uint64))
+
+
+def test_generator_gravity_frames_sets_exact_axis_sizes():
+    F = 129
+    mask = np.zeros(F, bool)
+    mask[[0, 5, 64, 127, 128]] = True
+    flat, _ = synthesize_rotation_averaging(F, 10, seed=1, gravity_frames=mask)
+    assert np.array_equal(flat.frame_dof == 1, mask)
+    assert flat.gauge_frame == 0
+    one = mask[flat.pair_frame1] & mask[flat.pair_frame2]
+    assert np.array_equal(flat.pair_dof == 1, one)
+    allg, _ = synthesize_rotation_averaging(20, 6, seed=1, gravity_frames=np.ones(20, bool))
+    assert (allg.frame_dof == 1).all() and (allg.pair_dof == 1).all() and allg.num_params == 20
+    with pytest.raises(ValueError):
+        synthesize_rotation_averaging(F, 10, seed=1, gravity_frames=mask[:-1])
