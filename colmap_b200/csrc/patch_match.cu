@@ -242,6 +242,28 @@ __global__ void pm_init_kernel(const PmParams P, float* sel_prev) {
 // NCC of one (hypothesis, source image) pair by an 8-lane group
 // (PhotoConsistencyCostComputer::Compute, patch_match_cuda.cu:489-593)
 // ------------------------------------------------------------------------------------------------
+// Phases of the pixel pass.  A build with -DPM_PIXEL_PHASES (tools/pm_pixel_phases.py; never the library build())
+// adds the clock() cycles lane 0 of every pixel-pass warp spends in each phase to pm_phase_cycles[pruned][phase]; in
+// every other build the phase marks are PmNoPhase and compile to nothing.
+enum { PM_PH_WAIT, PM_PH_SETUP, PM_PH_SELECT, PM_PH_TAPS, PM_PH_FINAL, PM_PH_BOUND, PM_PH_OTHER, PM_PH_COUNT };
+struct PmNoPhase {
+  __device__ __forceinline__ void operator()(int) const {}
+};
+#ifdef PM_PIXEL_PHASES
+__device__ unsigned long long pm_phase_cycles[2][PM_PH_COUNT];
+// mark(k): the cycles since the previous mark belong to phase k.  State in shared memory, one row per warp.
+struct PmPhaseClock {
+  unsigned long long* acc;
+  unsigned* last;
+  __device__ __forceinline__ void operator()(int k) const {
+    if ((threadIdx.x & 31) == 0) {
+      const unsigned now = (unsigned)clock();
+      acc[k] += now - *last;
+      *last = now;
+    }
+  }
+};
+#endif
 // Lane `sub` adds taps sub, sub + 8, ... in ascending order.  The loop is a software pipeline of depth D: the quad words
 // of the lane's next D - 1 taps are in flight while a tap is blended, so a warp waits on one gather latency per D taps
 // instead of one per tap.  The look-ahead index is clamped to the lane's last tap (the extra loads of the last
@@ -250,11 +272,15 @@ __global__ void pm_init_kernel(const PmParams P, float* sel_prev) {
 // (DESIGN.md §2 has the grid): the pixel pass <3, 3> (P 12.65 ms per sweep against 13.43 with the loop it replaced;
 // every U = 1 point and D = 4 lost, as did 7 and 6 resident CTAs); the serial pass and the initial cost <1, 5>, where
 // ptxas already overlaps the loads of the unrolled copies (S at D = 2 or 3 took 13.4-17.2 ms per sweep against 12.2).
-template <int D, int UNROLL>
-__device__ __forceinline__ float pm_ncc_group(const float4* __restrict__ patch, int ntaps, const float* __restrict__ pose,
+// The patch is read as two float2 arrays, tap t at wr[PS * t] ({w, w * ref}) and off[PS * t] ({dx, dy}): PS = 2 for the
+// interleaved float4 patch {w, w * ref, dx, dy} (off = wr + 1), PS = 1 for a split patch with a per-CTA offset table.
+template <int D, int UNROLL, int PS, class Phase = PmNoPhase>
+__device__ __forceinline__ float pm_ncc_group(const float2* __restrict__ wrp, const float2* __restrict__ offp, int ntaps,
+                                              const float* __restrict__ pose,
                                               const float iK[4], const uint32_t* __restrict__ quads, int pitch, int W,
                                               int H, float rowf, float colf, float d, float n0, float n1, float n2,
-                                              float inv_wsum, float rsum, float rsq, int sub, unsigned gmask) {
+                                              float inv_wsum, float rsum, float rsq, int sub, unsigned gmask,
+                                              Phase phase = Phase()) {
   float Hm[9];
   pm_compose_homography(pose, iK, rowf, colf, d, n0, n1, n2, Hm);
   const uint32_t* quads0 = quads + (2 * pitch + 2);
@@ -266,7 +292,7 @@ __device__ __forceinline__ float pm_ncc_group(const float4* __restrict__ patch, 
   const float cy = fmaf(Hm[3], colf, fmaf(Hm[4], rowf, Hm[5]));
   const float cz = fmaf(Hm[6], colf, fmaf(Hm[7], rowf, Hm[8]));
   auto fetch = [&](int t) {
-    const float2 off = reinterpret_cast<const float2*>(&patch[t])[1];   // {dx, dy} of {w, w * ref, dx, dy}
+    const float2 off = offp[PS * t];
     const float zx = fmaf(Hm[0], off.x, fmaf(Hm[1], off.y, cx));
     const float zy = fmaf(Hm[3], off.x, fmaf(Hm[4], off.y, cy));
     const float zz = fmaf(Hm[6], off.x, fmaf(Hm[7], off.y, cz));
@@ -275,12 +301,13 @@ __device__ __forceinline__ float pm_ncc_group(const float4* __restrict__ patch, 
   };
   auto consume = [&](int t, const PmQuadTap& q) {
     const float color = pm_quad_blend(q);
-    const float2 wr = reinterpret_cast<const float2*>(&patch[t])[0];    // {w, w * ref}
+    const float2 wr = wrp[PS * t];
     const float ws = wr.x * color;
     s1 += ws;
     s2 = fmaf(ws, color, s2);
     s3 = fmaf(wr.y, color, s3);
   };
+  phase(PM_PH_FINAL);   // the homography counts with the finalize: both are paid once per NCC
   const int cnt = (ntaps >> 3) + ((sub < (ntaps & 7)) ? 1 : 0);
   const int last = sub + 8 * (cnt > 0 ? cnt - 1 : 0);
   PmQuadTap st[D];
@@ -294,26 +321,30 @@ __device__ __forceinline__ float pm_ncc_group(const float4* __restrict__ patch, 
 #pragma unroll
     for (int k = 0; k < D - 1; ++k) st[k] = st[k + 1];
   }
+  phase(PM_PH_TAPS);
 #pragma unroll
   for (int o = 1; o < 8; o <<= 1) {
     s1 = s1 + __shfl_xor_sync(gmask, s1, o);
     s2 = s2 + __shfl_xor_sync(gmask, s2, o);
     s3 = s3 + __shfl_xor_sync(gmask, s3, o);
   }
-  return pm_ncc_finalize(s1, s2, s3, inv_wsum, rsum, rsq);
+  const float ncc = pm_ncc_finalize(s1, s2, s3, inv_wsum, rsum, rsq);
+  phase(PM_PH_FINAL);
+  return ncc;
 }
 
 
 // TransformPDFToCDF (:683-696) over the per-image lanes: sum in image order, then the running sum of prob / sum.
 // For N <= 8 the N values are fetched once and both passes run on registers (lanes >= N hold prob = 0: adding +0.0
 // changes nothing, so the loops can run over all 8 slots); same operations in the same order as the plain loops.
-__device__ __forceinline__ float pm_cdf_lanes(float prob, int N, int lane) {
+// width 8 (N <= 8 only): each 8-lane segment is one pixel, `lane` is the lane within the segment.
+__device__ __forceinline__ float pm_cdf_lanes(float prob, int N, int lane, int width = 32) {
   const unsigned full = 0xffffffffu;
   float cdf = 0.0f;
   if (N <= 8) {
     float pv[8];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) pv[i] = __shfl_sync(full, prob, i);
+    for (int i = 0; i < 8; ++i) pv[i] = __shfl_sync(full, prob, i, width);
     float sum = 0.0f;
 #pragma unroll
     for (int i = 0; i < 8; ++i) sum += pv[i];
@@ -335,14 +366,14 @@ __device__ __forceinline__ float pm_cdf_lanes(float prob, int N, int lane) {
   }
   return cdf;
 }
-// index of the first image whose CDF value exceeds u (-1: none), per lane
-__device__ __forceinline__ int pm_sample_image(float cdf, float u, int N) {
+// index of the first image whose CDF value exceeds u (-1: none), per lane; width as in pm_cdf_lanes
+__device__ __forceinline__ int pm_sample_image(float cdf, float u, int N, int width = 32) {
   const unsigned full = 0xffffffffu;
   int img = -1;
   if (N <= 8) {
 #pragma unroll
     for (int i = 7; i >= 0; --i) {
-      const float ci = __shfl_sync(full, cdf, i);
+      const float ci = __shfl_sync(full, cdf, i, width);
       if (i < N && ci > u) img = i;     // descending i: the smallest qualifying index wins
     }
   } else {
@@ -354,17 +385,19 @@ __device__ __forceinline__ int pm_sample_image(float cdf, float u, int N) {
   return img;
 }
 
-// reference patch of one pixel: bilateral weights + weighted colours + 1/sum(w); executed by one warp.
+// reference patch of one pixel: bilateral weights + weighted colours + 1/sum(w); executed by one warp.  Patch layout as in
+// pm_ncc_group.
+template <int PS>
 __device__ __forceinline__ void pm_build_patch(const PmParams& P, const float* lut, int rot, int fw, int fh, int row, int col,
-                                               float4* patch, int lane, float* inv_wsum_out) {
+                                               const float2* off, float2* wr, int lane, float* inv_wsum_out) {
   const float center = pm_ref_color(P, lut, rot, fw, fh, row, col);
   float partial = 0.0f;
   for (int t = lane; t < P.ntaps; t += 32) {
-    const float4 tp = patch[t];
-    const int dc = (int)tp.z, dr = (int)tp.w;
+    const float2 o = off[PS * t];
+    const int dc = (int)o.x, dr = (int)o.y;
     const float c = pm_ref_color(P, lut, rot, fw, fh, row + dr, col + dc);
     const float bw = pm_bilateral_weight(P.spatial_norm, P.color_norm, dr, dc, center, c);
-    reinterpret_cast<float2*>(&patch[t])[0] = make_float2(bw, bw * c);
+    wr[PS * t] = make_float2(bw, bw * c);
     partial += bw;
   }
 #pragma unroll
@@ -439,10 +472,14 @@ __global__ void __launch_bounds__(128) pm_patch_kernel(const PmParams P) {
 // Copy of pixel p's stored block into patch[t].xy in frame order (tsrc from pm_fill_tap_src): one 8-byte cp.async per
 // tap, so the copy is in flight while the issuing warp does other work.  The taps of a frame are a permutation of the
 // stored order, so every lane writes its own slot; the 121 x 8 B a warp reads are one contiguous block.
-__device__ __forceinline__ void pm_copy_patch(const PmParams& P, const int* tsrc, size_t p, float4* patch, int lane) {
+// the two halves of an interleaved patch entry {w, w * ref, dx, dy}
+__device__ __forceinline__ float2* pm_wr(float4* patch) { return reinterpret_cast<float2*>(patch); }
+__device__ __forceinline__ const float2* pm_off(const float4* patch) { return reinterpret_cast<const float2*>(patch) + 1; }
+template <int PS>
+__device__ __forceinline__ void pm_copy_patch(const PmParams& P, const int* tsrc, size_t p, float2* wr, int lane) {
   const float2* blk = P.patch_store + p * P.ntaps_st;
   for (int t = lane; t < P.ntaps; t += 32) {
-    const unsigned dst = (unsigned)__cvta_generic_to_shared(&patch[t]);
+    const unsigned dst = (unsigned)__cvta_generic_to_shared(&wr[PS * t]);
     asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"(dst), "l"(blk + tsrc[t]) : "memory");
   }
 }
@@ -474,11 +511,11 @@ __global__ void __launch_bounds__(128) pm_initial_cost_kernel(const PmParams P) 
     const int row = (int)(p / P.W0), col = (int)(p - (size_t)row * P.W0);
     float inv_wsum;
     if (P.patch_store) {
-      pm_copy_patch(P, tsrc, p, patch, lane);
+      pm_copy_patch<2>(P, tsrc, p, pm_wr(patch), lane);
       inv_wsum = P.patch_inv[p * 4];
       pm_copy_wait();
     } else {
-      pm_build_patch(P, lut, 0, P.W0, P.H0, row, col, patch, lane, &inv_wsum);
+      pm_build_patch<2>(P, lut, 0, P.W0, P.H0, row, col, pm_off(patch), pm_wr(patch), lane, &inv_wsum);
     }
     __syncwarp();
     const float4 hy = P.hyp[p];
@@ -487,7 +524,7 @@ __global__ void __launch_bounds__(128) pm_initial_cost_kernel(const PmParams P) 
       const int img = base + g;
       if (img < N) {
         const PmSrcDesc sd = P.src[img];
-        const float c = pm_ncc_group<1, 5>(patch, P.ntaps, poses + img * PM_POSE_STRIDE, P.invK[0], P.quads + sd.quad_off,
+        const float c = pm_ncc_group<1, 5, 2>(pm_wr(patch), pm_off(patch), P.ntaps, poses + img * PM_POSE_STRIDE, P.invK[0], P.quads + sd.quad_off,
                                      sd.pitch, sd.w, sd.h, (float)row, (float)col, hy.x, hy.y, hy.z, hy.w, inv_wsum,
                                      rsum, rsq, sub, gmask);
         if (sub == 0) P.cost[p * N + img] = c;
@@ -504,7 +541,8 @@ __global__ void __launch_bounds__(128) pm_initial_cost_kernel(const PmParams P) 
 //                        depend on the sweep's results, only on the hypotheses of the previous sweep);
 //   M  pm_msg_kernel     one thread per (column, image), beside R: the column's HMM messages over the
 //                        costs the sweep starts with;
-//   P  pm_pixel_kernel   pixel-parallel, one warp per pixel: everything that does not depend on the row
+//   P  pm_pixel_kernel   pixel-parallel, one warp per pixel (pm_pixel4_kernel for N <= 8: four pixels per warp
+//                        in the set-up, then one after the other): everything that does not depend on the row
 //                        above — the NCC of hypotheses 2..4 (rand/rand, cur/rand-normal, rand-depth/cur)
 //                        against every source image, the per-image priors, geometric costs;
 //   S  pm_serial_kernel  one CTA per column: propagation, HMM messages, Monte-Carlo sampling, the NCC
@@ -611,6 +649,18 @@ __global__ void __launch_bounds__(128, 8) pm_pixel_kernel(const PmParams P, cons
   const int ns = P.num_samples, nsl = ns < 32 ? ns : 32;
   const int mode = PRUNE ? A.prune : 0;
   (void)fw; (void)nsl; (void)full; (void)nmask;
+#ifdef PM_PIXEL_PHASES
+  __shared__ unsigned long long ph_acc[4][PM_PH_COUNT];
+  __shared__ unsigned ph_last[4];
+  if (lane == 0) {
+    for (int k = 0; k < PM_PH_COUNT; ++k) ph_acc[warp][k] = 0ull;
+    ph_last[warp] = (unsigned)clock();
+  }
+  __syncwarp();
+  const PmPhaseClock ph{ph_acc[warp], &ph_last[warp]};
+#else
+  const PmNoPhase ph;
+#endif
   // (an SM-local tiling of the pixel order was measured: L1 hit rate 67% -> 55%, slower; plain grid stride kept)
   for (size_t q = (size_t)blockIdx.x * 4 + warp; q < npix; q += (size_t)gridDim.x * 4) {
     const int row = (int)(q / fw), col = (int)(q - (size_t)row * fw);  // sweep-frame pixel
@@ -618,11 +668,12 @@ __global__ void __launch_bounds__(128, 8) pm_pixel_kernel(const PmParams P, cons
     const float rowf = (float)row, colf = (float)col;
     float inv_wsum;
     if (P.patch_store) {   // in flight while the pixel's inputs load and its priors are computed
-      pm_copy_patch(P, tsrc, p, patch, lane);
+      pm_copy_patch<2>(P, tsrc, p, pm_wr(patch), lane);
       inv_wsum = P.patch_inv[p * 4 + rot];
     } else {
-      pm_build_patch(P, lut, rot, fw, fh, row, col, patch, lane, &inv_wsum);
+      pm_build_patch<2>(P, lut, rot, fw, fh, row, col, pm_off(patch), pm_wr(patch), lane, &inv_wsum);
     }
+    ph(PM_PH_OTHER);
     const float4 cur4 = P.hyp[p];
     float cn0 = cur4.y, cn1 = cur4.z;
     pm_normal_to_frame(rot, cn0, cn1);
@@ -656,7 +707,9 @@ __global__ void __launch_bounds__(128, 8) pm_pixel_kernel(const PmParams P, cons
         prob = sp * pt * pi * pr;
       }
     }
+    ph(PM_PH_SETUP);
     pm_copy_wait();
+    ph(PM_PH_WAIT);
     if (!PRUNE) {   // every (hypothesis, image) pair, four per round
       __syncwarp();
       const int npairs = 3 * N;
@@ -667,9 +720,11 @@ __global__ void __launch_bounds__(128, 8) pm_pixel_kernel(const PmParams P, cons
           const float hd = (hsel == 1) ? cur_d : r4.x;
           const float hn0 = (hsel == 2) ? cn0 : r4.y, hn1 = (hsel == 2) ? cn1 : r4.z, hn2 = (hsel == 2) ? cn2 : r4.w;
           const PmSrcDesc sd = P.src[img];
-          const float c = pm_ncc_group<3, 3>(patch, P.ntaps, poses + img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch,
-                                       sd.w, sd.h, rowf, colf, hd, hn0, hn1, hn2, inv_wsum, rsum, rsq, sub, gmask);
+          ph(PM_PH_SELECT);
+          const float c = pm_ncc_group<3, 3, 2>(pm_wr(patch), pm_off(patch), P.ntaps, poses + img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch,
+                                       sd.w, sd.h, rowf, colf, hd, hn0, hn1, hn2, inv_wsum, rsum, rsq, sub, gmask, ph);
           if (sub == 0) A.tab3[(p * 3 + hsel) * N + img] = c;
+          ph(PM_PH_FINAL);
         }
       }
       __syncwarp();
@@ -700,6 +755,7 @@ __global__ void __launch_bounds__(128, 8) pm_pixel_kernel(const PmParams P, cons
     } else if (mode != 0) {
       act0 = act1 = act2 = false;
     }
+    ph(PM_PH_SETUP);
     float L0 = 0.0f, L1 = 0.0f, L2 = 0.0f;
     while (act0 || act1 || act2) {
       // up to four (hypothesis, image) pairs per round, hypotheses taking turns, images by multiplicity
@@ -721,15 +777,17 @@ __global__ void __launch_bounds__(128, 8) pm_pixel_kernel(const PmParams P, cons
           }
         }
       }
+      ph(PM_PH_SELECT);
       if (slot == 0) break;
       float c = 0.0f;
       if (my_k >= 0) {   // hsel 0: rand/rand, 1: cur depth + rand normal, 2: rand depth + cur normal
         const float hd = (my_k == 1) ? cur_d : r4.x;
         const float hn0 = (my_k == 2) ? cn0 : r4.y, hn1 = (my_k == 2) ? cn1 : r4.z, hn2 = (my_k == 2) ? cn2 : r4.w;
         const PmSrcDesc sd = P.src[my_img];
-        c = pm_ncc_group<3, 3>(patch, P.ntaps, poses + my_img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch, sd.w, sd.h,
-                         rowf, colf, hd, hn0, hn1, hn2, inv_wsum, rsum, rsq, sub, gmask);
+        c = pm_ncc_group<3, 3, 2>(pm_wr(patch), pm_off(patch), P.ntaps, poses + my_img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch, sd.w, sd.h,
+                         rowf, colf, hd, hn0, hn1, hn2, inv_wsum, rsum, rsq, sub, gmask, ph);
         if (sub == 0) A.tab3[(p * 3 + my_k) * N + my_img] = c;
+        ph(PM_PH_FINAL);
       }
       if (mode == 1) {
 #pragma unroll
@@ -748,9 +806,245 @@ __global__ void __launch_bounds__(128, 8) pm_pixel_kernel(const PmParams P, cons
       } else {
         act0 = rem0 != 0u; act1 = rem1 != 0u; act2 = rem2 != 0u;
       }
+      ph(PM_PH_BOUND);
     }
     __syncwarp();
   }
+#ifdef PM_PIXEL_PHASES
+  if (lane == 0)
+    for (int k = 0; k < PM_PH_COUNT; ++k) atomicAdd(&pm_phase_cycles[PRUNE ? 1 : 0][k], ph_acc[warp][k]);
+#endif
+}
+
+// P for N <= 8: a warp takes a batch of four consecutive pixels (by index in the sweep frame, so a batch may run over
+// a row end) and lane (g, sub) = (lane >> 3, lane & 7) does the set-up of pixel g against image sub: the priors,
+// the geometric costs, the selection probability, the CDF and the sample prediction of all four pixels at once (the
+// kernel above runs them on N of 32 lanes, once per pixel).  The same functions on the same values, so prior3 / gtab2
+// hold the same bits.  The NCC rounds then take the four pixels one after the other, each with the schedule and the
+// early-out rules of the kernel above.  Shared memory: the four reference patches of a warp as {w, w * ref} (8 B per
+// tap and pixel) and one {dx, dy} table per CTA: 8 * 17 * ntaps_pad + 4 * (43 N + ntaps_pad + 256) bytes, 20.3 KB at
+// C2 (window 11, N = 8), so 8 CTAs still fit an SM.
+template <bool GEOM, bool PRUNE>
+__global__ void __launch_bounds__(128, 8) pm_pixel4_kernel(const PmParams P, const PmSweepArgs A) {
+  extern __shared__ float4 smem4[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int rot = A.rot, N = P.N, tp = P.ntaps_pad;
+  const int fw = (rot & 1) ? P.H0 : P.W0, fh = (rot & 1) ? P.W0 : P.H0;
+  float2* wr_warp = reinterpret_cast<float2*>(smem4) + (size_t)warp * 4 * tp;   // [4 pixels][ntaps_pad] {w, w * ref}
+  float2* off = reinterpret_cast<float2*>(smem4) + 16 * tp;                     // [ntaps_pad] {dx, dy}
+  float* poses = reinterpret_cast<float*>(off + tp);
+  int* tsrc = reinterpret_cast<int*>(poses + N * PM_POSE_STRIDE);
+  float* lut = reinterpret_cast<float*>(tsrc + tp);
+  for (int i = threadIdx.x; i < N * PM_POSE_STRIDE; i += blockDim.x) poses[i] = P.poses[(size_t)rot * N * PM_POSE_STRIDE + i];
+  for (int t = threadIdx.x; t < tp; t += blockDim.x) {   // pm_fill_tap_offsets' {dx, dy}
+    const int tr = t / P.nside, tc = t - tr * P.nside;
+    off[t] = make_float2((float)(-P.radius + P.step * tc), (float)(-P.radius + P.step * tr));
+  }
+  pm_fill_tap_src(P, rot, tsrc, threadIdx.x, blockDim.x);
+  pm_load_lut(lut, threadIdx.x, blockDim.x);
+  const float iK[4] = {P.invK[rot][0], P.invK[rot][1], P.invK[rot][2], P.invK[rot][3]};
+  const float Kr[4] = {P.K[rot][0], P.K[rot][1], P.K[rot][2], P.K[rot][3]};
+  __syncthreads();
+  const size_t npix = (size_t)fw * fh;
+  const int g = lane >> 3, sub = lane & 7;
+  const unsigned gmask = 0xffu << (8 * g);
+  const unsigned full = 0xffffffffu;
+  const unsigned nmask = (1u << N) - 1u;
+  const int ns = P.num_samples, nsl = ns < 32 ? ns : 32;
+  const int mode = PRUNE ? A.prune : 0;
+  const bool img_lane = sub < N;
+  (void)nsl; (void)nmask;
+#ifdef PM_PIXEL_PHASES
+  __shared__ unsigned long long ph_acc[4][PM_PH_COUNT];
+  __shared__ unsigned ph_last[4];
+  if (lane == 0) {
+    for (int k = 0; k < PM_PH_COUNT; ++k) ph_acc[warp][k] = 0ull;
+    ph_last[warp] = (unsigned)clock();
+  }
+  __syncwarp();
+  const PmPhaseClock ph{ph_acc[warp], &ph_last[warp]};
+#else
+  const PmNoPhase ph;
+#endif
+  for (size_t q0 = ((size_t)blockIdx.x * 4 + warp) * 4; q0 < npix; q0 += (size_t)gridDim.x * 16) {
+    const int npx = (int)min((size_t)4, npix - q0);   // pixels of the batch inside the frame
+    const bool live = g < npx;
+    const size_t q = live ? q0 + g : q0;              // a group past the frame's end repeats pixel q0 and stores nothing
+    const int row = (int)(q / fw), col = (int)(q - (size_t)row * fw);
+    const size_t p = pm_pix0(P.W0, P.H0, rot, row, col);
+    const float rowf = (float)row, colf = (float)col;
+    float inv_wsum = 0.0f;
+    for (int k = 0; k < npx; ++k) {   // the batch's patches: copies in flight while the set-up below runs
+      const int rk = __shfl_sync(full, row, 8 * k), ck = __shfl_sync(full, col, 8 * k);
+      if (P.patch_store) {
+        pm_copy_patch<1>(P, tsrc, pm_pix0(P.W0, P.H0, rot, rk, ck), wr_warp + k * tp, lane);
+      } else {
+        float iw;
+        pm_build_patch<1>(P, lut, rot, fw, fh, rk, ck, off, wr_warp + k * tp, lane, &iw);
+        if (g == k) inv_wsum = iw;
+      }
+    }
+    if (P.patch_store) inv_wsum = P.patch_inv[p * 4 + rot];
+    ph(PM_PH_OTHER);
+    const float4 cur4 = P.hyp[p];
+    float cn0 = cur4.y, cn1 = cur4.z;
+    pm_normal_to_frame(rot, cn0, cn1);
+    const float cur_d = cur4.x, cn2 = cur4.w;
+    const float4 r4 = A.rand_hyp[p];
+    const float rsum = P.ref_sum[p], rsq = P.ref_sqsum[p];
+    float prob = 0.0f, cost_i = 0.0f, gcur = 0.0f, grand = 0.0f;
+    if (img_lane) {  // per-image priors of the current hypothesis (:1079-1103)
+      const float* pose = poses + sub * PM_POSE_STRIDE;
+      const float rx = fmaf(iK[0], colf, iK[1]), ry = fmaf(iK[2], rowf, iK[3]);
+      float ct, ci;
+      pm_viewing_angles(pose, cur_d * rx, cur_d * ry, cur_d, cn0, cn1, cn2, &ct, &ci);
+      float Hm[9];
+      pm_compose_homography(pose, iK, rowf, colf, cur_d, cn0, cn1, cn2, Hm);
+      // kept as three factors: the serial pass evaluates sel_prob * tri * inc * res left to right (:1103)
+      const float pt = pm_tri_prob(P.L, ct), pi = pm_inc_prob(P.L, ci), pr = pm_res_prob(Hm, rowf, colf, P.radius);
+      if (live) {
+        A.prior3[(p * 3 + 0) * N + sub] = pt;
+        A.prior3[(p * 3 + 1) * N + sub] = pi;
+        A.prior3[(p * 3 + 2) * N + sub] = pr;
+      }
+      if (GEOM) {
+        const PmSrcDesc sd = P.src[sub];
+        const float* dm = P.src_depth + sd.depth_off;
+        gcur = pm_geom_cost(pose, Kr, iK, dm, sd.w, sd.h, rowf, colf, cur_d, P.geom_max_cost);
+        grand = pm_geom_cost(pose, Kr, iK, dm, sd.w, sd.h, rowf, colf, r4.x, P.geom_max_cost);
+        if (live) {
+          A.gtab2[(p * 2 + 0) * N + sub] = gcur;
+          A.gtab2[(p * 2 + 1) * N + sub] = grand;
+        }
+      }
+      if (mode == 1) {
+        cost_i = P.cost[p * N + sub];
+        const float sp = pm_sel_prob(A.fwd_pred[p * N + sub], A.sel_cur[p * N + sub], A.sel_prev[p * N + sub], A.prev_w);
+        prob = sp * pt * pi * pr;
+      }
+    }
+    // ---- which images will be sampled, and how often (prediction; mode 0: every image once), per 8-lane segment
+    int mult = img_lane ? 1 : 0;
+    unsigned needed4 = 0u;   // bits 8k..8k+7: images pixel k samples
+    float thr = 3.0e38f;
+    if (PRUNE) {
+      if (live)
+        for (int e = sub; e < 3 * N; e += 8) A.tab3[p * 3 * N + e] = PM_NOT_EVALUATED;
+      if (mode == 1) {
+        const float cdf = pm_cdf_lanes(prob, N, sub, 8);
+        mult = 0;
+        for (int s0 = 0; s0 < nsl; s0 += 8) {   // lane sub predicts sample s0 + sub of its pixel
+          const float u = (s0 + sub < nsl) ? A.usamp[p * ns + s0 + sub] : 2.0f;
+          const int img = pm_sample_image(cdf, u, N, 8);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) mult += (__shfl_sync(full, img, j, 8) == sub) ? 1 : 0;
+        }
+        if (!img_lane) mult = 0;
+        needed4 = __ballot_sync(full, live && mult > 0);
+        float t = (float)mult * (GEOM ? fmaf(P.geom_reg, gcur, cost_i) : cost_i);
+#pragma unroll
+        for (int o = 4; o > 0; o >>= 1) t += __shfl_xor_sync(full, t, o);
+        thr = fmaf(t, 1.001f, 1e-3f);   // predicted cost sum of the current hypothesis, with a margin for the true order of summation
+      }
+    }
+    ph(PM_PH_SETUP);
+    pm_copy_wait();
+    __syncwarp();   // patches complete; sentinel stores ordered before the result stores of other lanes
+    ph(PM_PH_WAIT);
+    for (int k = 0; k < npx; ++k) {
+      // pixel k's values, from the lanes of segment k (image-indexed ones to lane == image)
+      const int src = 8 * k + sub;
+      const float krow = __shfl_sync(full, rowf, 8 * k), kcol = __shfl_sync(full, colf, 8 * k);
+      const float kd = __shfl_sync(full, cur_d, 8 * k), kn0 = __shfl_sync(full, cn0, 8 * k), kn1 = __shfl_sync(full, cn1, 8 * k),
+                  kn2 = __shfl_sync(full, cn2, 8 * k);
+      const float rd = __shfl_sync(full, r4.x, 8 * k), rn0 = __shfl_sync(full, r4.y, 8 * k), rn1 = __shfl_sync(full, r4.z, 8 * k),
+                  rn2 = __shfl_sync(full, r4.w, 8 * k);
+      const float kiw = __shfl_sync(full, inv_wsum, 8 * k), krs = __shfl_sync(full, rsum, 8 * k), krq = __shfl_sync(full, rsq, 8 * k);
+      const size_t kp = pm_pix0(P.W0, P.H0, rot, (int)krow, (int)kcol);
+      const float2* kwr = wr_warp + k * tp;
+      auto ncc = [&](int hsel, int img) {   // hsel 0: rand/rand, 1: cur depth + rand normal, 2: rand depth + cur normal
+        const float hd = (hsel == 1) ? kd : rd;
+        const float hn0 = (hsel == 2) ? kn0 : rn0, hn1 = (hsel == 2) ? kn1 : rn1, hn2 = (hsel == 2) ? kn2 : rn2;
+        const PmSrcDesc sd = P.src[img];
+        const float c = pm_ncc_group<3, 3, 1>(kwr, off, P.ntaps, poses + img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch,
+                                              sd.w, sd.h, krow, kcol, hd, hn0, hn1, hn2, kiw, krs, krq, sub, gmask, ph);
+        if (sub == 0) A.tab3[(kp * 3 + hsel) * N + img] = c;
+        ph(PM_PH_FINAL);
+        return c;
+      };
+      if (!PRUNE) {   // every (hypothesis, image) pair, four per round
+        const int npairs = 3 * N;
+        for (int base = 0; base < npairs; base += 4) {
+          const int pair = base + g;
+          ph(PM_PH_SELECT);
+          if (pair < npairs) ncc(pair / N, pair % N);
+        }
+        continue;
+      }
+      const int kmult = __shfl_sync(full, mult, src);   // lanes 0..7: multiplicity of image lane
+      const float kthr = __shfl_sync(full, thr, 8 * k);
+      const float kgc = GEOM ? __shfl_sync(full, gcur, src) : 0.0f, kgr = GEOM ? __shfl_sync(full, grand, src) : 0.0f;
+      const unsigned needed = (needed4 >> (8 * k)) & 0xffu;
+      unsigned rem0 = nmask, rem1 = nmask, rem2 = nmask, ev0 = 0u, ev1 = 0u, ev2 = 0u;
+      bool act0 = true, act1 = true, act2 = true, ext0 = true, ext1 = true, ext2 = true;
+      if (mode == 1) {
+        rem0 = rem1 = rem2 = needed;
+        ext0 = ext1 = ext2 = false;
+        act0 = act1 = act2 = needed != 0u;
+      } else if (mode != 0) {
+        act0 = act1 = act2 = false;
+      }
+      float L0 = 0.0f, L1 = 0.0f, L2 = 0.0f;
+      while (act0 || act1 || act2) {
+        // up to four (hypothesis, image) pairs per round, hypotheses taking turns, images by multiplicity
+        int my_k = -1, my_img = 0, slot = 0;
+#pragma unroll
+        for (int pass = 0; pass < 2; ++pass) {
+#pragma unroll
+          for (int h = 0; h < 3; ++h) {
+            const bool a = (h == 0) ? act0 : ((h == 1) ? act1 : act2);
+            const unsigned rem = (h == 0) ? rem0 : ((h == 1) ? rem1 : rem2);
+            if (slot < 4 && a && rem) {
+              const unsigned key = ((rem >> lane) & 1u) ? ((((unsigned)kmult) << 5) | (unsigned)(31 - lane)) + 1u : 0u;
+              const unsigned best = __reduce_max_sync(full, key);
+              const int im = 31 - (int)((best - 1u) & 31u);
+              const unsigned bit = 1u << im;
+              if (h == 0) { rem0 &= ~bit; ev0 |= bit; } else if (h == 1) { rem1 &= ~bit; ev1 |= bit; } else { rem2 &= ~bit; ev2 |= bit; }
+              if (slot == g) { my_k = h; my_img = im; }
+              ++slot;
+            }
+          }
+        }
+        ph(PM_PH_SELECT);
+        if (slot == 0) break;
+        float c = 0.0f;
+        if (my_k >= 0) c = ncc(my_k, my_img);
+        if (mode == 1) {
+#pragma unroll
+          for (int s2 = 0; s2 < 4; ++s2) {
+            const int ks = __shfl_sync(full, my_k, 8 * s2), is = __shfl_sync(full, my_img, 8 * s2);
+            float v = __shfl_sync(full, c, 8 * s2);
+            const float w = (float)__shfl_sync(full, kmult, is & 31);
+            if (GEOM) v = fmaf(P.geom_reg, __shfl_sync(full, (ks == 1) ? kgc : kgr, is & 31), v);
+            if (ks == 0) L0 = fmaf(w, v, L0); else if (ks == 1) L1 = fmaf(w, v, L1); else if (ks == 2) L2 = fmaf(w, v, L2);
+          }
+          // a hypothesis whose partial sum already exceeds the current hypothesis' sum is out; one that survives all its
+          // sampled images is a likely winner: the images nobody sampled are then needed for the cost map (:1184-1196)
+          if (act0) { if (L0 > kthr) act0 = false; else if (!rem0) { if (!ext0) { ext0 = true; rem0 = nmask & ~ev0; } if (!rem0) act0 = false; } }
+          if (act1) { if (L1 > kthr) act1 = false; else if (!rem1) { if (!ext1) { ext1 = true; rem1 = nmask & ~ev1; } if (!rem1) act1 = false; } }
+          if (act2) { if (L2 > kthr) act2 = false; else if (!rem2) { if (!ext2) { ext2 = true; rem2 = nmask & ~ev2; } if (!rem2) act2 = false; } }
+        } else {
+          act0 = rem0 != 0u; act1 = rem1 != 0u; act2 = rem2 != 0u;
+        }
+        ph(PM_PH_BOUND);
+      }
+    }
+    __syncwarp();   // every group is done with the batch's patches before the next batch's copies overwrite them
+  }
+#ifdef PM_PIXEL_PHASES
+  if (lane == 0)
+    for (int k = 0; k < PM_PH_COUNT; ++k) atomicAdd(&pm_phase_cycles[PRUNE ? 1 : 0][k], ph_acc[warp][k]);
+#endif
 }
 
 // STORE: the patch comes from the patch store (P.patch_store set).  A template parameter, not a runtime branch, so that
@@ -783,7 +1077,7 @@ __global__ void __launch_bounds__(32 * WPC, 16 / WPC) pm_serial_kernel(const PmP
   auto copy_row = [&](int row) {
     const size_t p = pm_pix0(P.W0, P.H0, rot, row, col);
     float* fc = fctl2 + 4 * (row & 1);
-    pm_copy_patch(P, tsrc, p, patch2 + (row & 1) * P.ntaps_pad, lane);
+    pm_copy_patch<2>(P, tsrc, p, pm_wr(patch2 + (row & 1) * P.ntaps_pad), lane);
     if (lane == 0) { pm_copy_scalar(fc, P.patch_inv + p * 4 + rot); pm_copy_scalar(fc + 1, P.ref_sum + p); pm_copy_scalar(fc + 2, P.ref_sqsum + p); }
   };
   const float iK[4] = {P.invK[rot][0], P.invK[rot][1], P.invK[rot][2], P.invK[rot][3]};
@@ -839,7 +1133,7 @@ __global__ void __launch_bounds__(32 * WPC, 16 / WPC) pm_serial_kernel(const PmP
         pm_copy_wait();
       } else {
         float inv_wsum;
-        pm_build_patch(P, lut, rot, fw, fh, row, col, patch, lane, &inv_wsum);
+        pm_build_patch<2>(P, lut, rot, fw, fh, row, col, pm_off(patch), pm_wr(patch), lane, &inv_wsum);
         if (lane == 0) { fctl[0] = inv_wsum; fctl[1] = P.ref_sum[p]; fctl[2] = P.ref_sqsum[p]; }
       }
     }
@@ -878,7 +1172,7 @@ __global__ void __launch_bounds__(32 * WPC, 16 / WPC) pm_serial_kernel(const PmP
       const float hd = hyp1[0], hn0 = hyp1[1], hn1 = hyp1[2], hn2 = hyp1[3];
       for (int img = warp * 4 + g; img < N; img += 4 * WPC) {
         const PmSrcDesc sd = P.src[img];
-        const float c = pm_ncc_group<1, 5>(patch, P.ntaps, poses + img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch,
+        const float c = pm_ncc_group<1, 5, 2>(pm_wr(patch), pm_off(patch), P.ntaps, poses + img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch,
                                      sd.w, sd.h, rowf, colf, hd, hn0, hn1, hn2, inv_wsum, rsum, rsq, sub, gmask);
         if (sub == 0) tab1[img] = c;
       }
@@ -907,7 +1201,7 @@ __global__ void __launch_bounds__(32 * WPC, 16 / WPC) pm_serial_kernel(const PmP
           float c = 0.0f;
           if (my_img >= 0) {
             const PmSrcDesc sd = P.src[my_img];
-            c = pm_ncc_group<1, 5>(patch, P.ntaps, poses + my_img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch, sd.w, sd.h,
+            c = pm_ncc_group<1, 5, 2>(pm_wr(patch), pm_off(patch), P.ntaps, poses + my_img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch, sd.w, sd.h,
                              rowf, colf, hd, hn0, hn1, hn2, inv_wsum, rsum, rsq, sub, gmask);
           }
 #pragma unroll
@@ -1103,6 +1397,7 @@ struct b200pm_context {
   int last_launches = 0;
   std::vector<int> src_image_idxs;
   size_t smem_init = 0, smem_serial = 0, smem_patch = 0;
+  size_t smem_pixel4 = 0;   // 0: the pixel pass runs pm_pixel_kernel (N > 8, or four split patches do not fit a CTA)
   size_t patch_store_bytes = 0;   // 0: the reference patches are built inline by every consumer
   float4* rand_hyp = nullptr; unsigned char* ntrials = nullptr; float* usamp = nullptr; float* prior3 = nullptr; float* tab3 = nullptr; float* gtab2 = nullptr;
   float* fwd_pred = nullptr;
@@ -1371,6 +1666,12 @@ int b200pm_create(const b200pm_options* o, const b200pm_problem* p, b200pm_handl
   c->smem_init = sizeof(float4) * 4 * P.ntaps_pad + sizeof(float) * ((size_t)N * PM_POSE_STRIDE + P.ntaps_pad + 256);
   c->smem_serial = sizeof(float4) * 2 * P.ntaps_pad + sizeof(float) * ((size_t)N * PM_POSE_STRIDE + 32 + 4 + 8 + 272 + P.ntaps_pad + 256);
   c->smem_patch = sizeof(float) * (256 + 9 * (size_t)P.ntaps_pad);   // lut, tap offsets (int2), 3 tap maps, 4 warps' weights
+  {   // pm_pixel4_kernel: 16 split patches, the {dx, dy} table, poses, tap map, /255 table
+    const size_t bytes = sizeof(float2) * 17 * P.ntaps_pad + sizeof(float) * ((size_t)N * PM_POSE_STRIDE + P.ntaps_pad + 256);
+    int optin = 0;
+    cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, c->device);
+    if (N <= 8 && bytes <= (size_t)optin) c->smem_pixel4 = bytes;
+  }
   const size_t store_bytes = n * ((size_t)P.ntaps_st * sizeof(float2) + 4 * sizeof(float));
   if (patch_store && store_bytes <= PM_PATCH_STORE_BUDGET) {
     PM_CUDA(pm_alloc(c, &P.patch_store, n * P.ntaps_st));
@@ -1425,6 +1726,12 @@ int b200pm_run(b200pm_handle c) {
     PM_CUDA(cudaFuncSetAttribute(pm_pixel_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_init));
     PM_CUDA(cudaFuncSetAttribute(pm_pixel_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_init));
     PM_CUDA(cudaFuncSetAttribute(pm_pixel_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_init));
+  }
+  if (c->smem_pixel4 > 48 * 1024) {
+    PM_CUDA(cudaFuncSetAttribute(pm_pixel4_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_pixel4));
+    PM_CUDA(cudaFuncSetAttribute(pm_pixel4_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_pixel4));
+    PM_CUDA(cudaFuncSetAttribute(pm_pixel4_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_pixel4));
+    PM_CUDA(cudaFuncSetAttribute(pm_pixel4_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_pixel4));
   }
   int launches = 0;
   PM_CUDA(cudaEventRecord(c->ev[0], s));
@@ -1482,7 +1789,14 @@ int b200pm_run(b200pm_handle c) {
       mark(1);
       const size_t npx = (size_t)fw * ((sweep & 1) ? P.W0 : P.H0);
       const int pgrid = (int)((npx + 4 * PM_PIXELS_PER_WARP - 1) / (4 * PM_PIXELS_PER_WARP));
-      if (P.geom) {
+      const size_t s4 = c->smem_pixel4;
+      if (s4 && P.geom) {
+        if (A.prune) pm_pixel4_kernel<true, true><<<pgrid, 128, s4, s>>>(P, A);
+        else pm_pixel4_kernel<true, false><<<pgrid, 128, s4, s>>>(P, A);
+      } else if (s4) {
+        if (A.prune) pm_pixel4_kernel<false, true><<<pgrid, 128, s4, s>>>(P, A);
+        else pm_pixel4_kernel<false, false><<<pgrid, 128, s4, s>>>(P, A);
+      } else if (P.geom) {
         if (A.prune) pm_pixel_kernel<true, true><<<pgrid, 128, c->smem_init, s>>>(P, A);
         else pm_pixel_kernel<true, false><<<pgrid, 128, c->smem_init, s>>>(P, A);
       } else {
@@ -1664,5 +1978,16 @@ void b200pm_test_homography(const float* pose, const float* iK, float row, float
   pm_compose_homography(pose, iK, row, col, depth, n[0], n[1], n[2], H);
 }
 int b200pm_test_border_index(int W0, int H0, int r0, int c0) { return pm_border_index(W0, H0, r0, c0); }
+
+#ifdef PM_PIXEL_PHASES
+// diagnostic build: out[pruned * PM_PH_COUNT + phase] = pixel-pass cycles since the last call, then reset
+int b200pm_debug_pixel_phases(unsigned long long* out) {
+  PM_CUDA(cudaDeviceSynchronize());
+  PM_CUDA(cudaMemcpyFromSymbol(out, pm_phase_cycles, sizeof(pm_phase_cycles)));
+  const unsigned long long zero[2][PM_PH_COUNT] = {};
+  PM_CUDA(cudaMemcpyToSymbol(pm_phase_cycles, zero, sizeof(zero)));
+  return PM_PH_COUNT;
+}
+#endif
 
 }  // extern "C"
