@@ -263,6 +263,13 @@ struct PmPhaseClock {
     }
   }
 };
+// pm_pool_counts[pruned][k], the same build only: k = 0 NCCs pm_pixel4_kernel evaluated, 1 its rounds (four group slots
+// each), 2 NCCs the serial pass evaluated itself (entries the pixel pass left out)
+enum { PM_CNT_P_NCC, PM_CNT_P_ROUNDS, PM_CNT_S_NCC, PM_CNT_COUNT };
+__device__ unsigned long long pm_pool_counts[2][PM_CNT_COUNT];
+#define PM_POOL_COUNT(var, v) ((var) += (v))
+#else
+#define PM_POOL_COUNT(var, v) ((void)0)
 #endif
 // Lane `sub` adds taps sub, sub + 8, ... in ascending order.  The loop is a software pipeline of depth D: the quad words
 // of the lane's next D - 1 taps are in flight while a tap is blended, so a warp waits on one gather latency per D taps
@@ -541,8 +548,8 @@ __global__ void __launch_bounds__(128) pm_initial_cost_kernel(const PmParams P) 
 //                        depend on the sweep's results, only on the hypotheses of the previous sweep);
 //   M  pm_msg_kernel     one thread per (column, image), beside R: the column's HMM messages over the
 //                        costs the sweep starts with;
-//   P  pm_pixel_kernel   pixel-parallel, one warp per pixel (pm_pixel4_kernel for N <= 8: four pixels per warp
-//                        in the set-up, then one after the other): everything that does not depend on the row
+//   P  pm_pixel_kernel   pixel-parallel, one warp per pixel (pm_pixel4_kernel for N <= 8: four pixels per warp,
+//                        their NCC rounds pooled): everything that does not depend on the row
 //                        above — the NCC of hypotheses 2..4 (rand/rand, cur/rand-normal, rand-depth/cur)
 //                        against every source image, the per-image priors, geometric costs;
 //   S  pm_serial_kernel  one CTA per column: propagation, HMM messages, Monte-Carlo sampling, the NCC
@@ -820,10 +827,11 @@ __global__ void __launch_bounds__(128, 8) pm_pixel_kernel(const PmParams P, cons
 // a row end) and lane (g, sub) = (lane >> 3, lane & 7) does the set-up of pixel g against image sub: the priors,
 // the geometric costs, the selection probability, the CDF and the sample prediction of all four pixels at once (the
 // kernel above runs them on N of 32 lanes, once per pixel).  The same functions on the same values, so prior3 / gtab2
-// hold the same bits.  The NCC rounds then take the four pixels one after the other, each with the schedule and the
-// early-out rules of the kernel above.  Shared memory: the four reference patches of a warp as {w, w * ref} (8 B per
-// tap and pixel) and one {dx, dy} table per CTA: 8 * 17 * ntaps_pad + 4 * (43 N + ntaps_pad + 256) bytes, 20.3 KB at
-// C2 (window 11, N = 8), so 8 CTAs still fit an SM.
+// hold the same bits.  The NCC rounds are pooled over the batch: a round's four group slots take pairs of any of the
+// four pixels, one per pixel and pass, and after each round every pixel applies the early-out rules of the kernel above
+// to its own results.  Which entries the pass fills changes, never their values.  Shared memory: the four reference
+// patches of a warp as {w, w * ref} (8 B per tap and pixel) and one {dx, dy} table per CTA:
+// 8 * 17 * ntaps_pad + 4 * (43 N + ntaps_pad + 256) bytes, 20.3 KB at C2 (window 11, N = 8), so 8 CTAs still fit an SM.
 template <bool GEOM, bool PRUNE>
 __global__ void __launch_bounds__(128, 8) pm_pixel4_kernel(const PmParams P, const PmSweepArgs A) {
   extern __shared__ float4 smem4[];
@@ -853,7 +861,7 @@ __global__ void __launch_bounds__(128, 8) pm_pixel4_kernel(const PmParams P, con
   const int ns = P.num_samples, nsl = ns < 32 ? ns : 32;
   const int mode = PRUNE ? A.prune : 0;
   const bool img_lane = sub < N;
-  (void)nsl; (void)nmask;
+  (void)nsl;
 #ifdef PM_PIXEL_PHASES
   __shared__ unsigned long long ph_acc[4][PM_PH_COUNT];
   __shared__ unsigned ph_last[4];
@@ -863,6 +871,7 @@ __global__ void __launch_bounds__(128, 8) pm_pixel4_kernel(const PmParams P, con
   }
   __syncwarp();
   const PmPhaseClock ph{ph_acc[warp], &ph_last[warp]};
+  unsigned long long n_ncc = 0ull, n_rounds = 0ull;
 #else
   const PmNoPhase ph;
 #endif
@@ -951,99 +960,120 @@ __global__ void __launch_bounds__(128, 8) pm_pixel4_kernel(const PmParams P, con
     pm_copy_wait();
     __syncwarp();   // patches complete; sentinel stores ordered before the result stores of other lanes
     ph(PM_PH_WAIT);
-    for (int k = 0; k < npx; ++k) {
-      // pixel k's values, from the lanes of segment k (image-indexed ones to lane == image)
-      const int src = 8 * k + sub;
-      const float krow = __shfl_sync(full, rowf, 8 * k), kcol = __shfl_sync(full, colf, 8 * k);
-      const float kd = __shfl_sync(full, cur_d, 8 * k), kn0 = __shfl_sync(full, cn0, 8 * k), kn1 = __shfl_sync(full, cn1, 8 * k),
-                  kn2 = __shfl_sync(full, cn2, 8 * k);
-      const float rd = __shfl_sync(full, r4.x, 8 * k), rn0 = __shfl_sync(full, r4.y, 8 * k), rn1 = __shfl_sync(full, r4.z, 8 * k),
-                  rn2 = __shfl_sync(full, r4.w, 8 * k);
-      const float kiw = __shfl_sync(full, inv_wsum, 8 * k), krs = __shfl_sync(full, rsum, 8 * k), krq = __shfl_sync(full, rsq, 8 * k);
-      const size_t kp = pm_pix0(P.W0, P.H0, rot, (int)krow, (int)kcol);
-      const float2* kwr = wr_warp + k * tp;
-      auto ncc = [&](int hsel, int img) {   // hsel 0: rand/rand, 1: cur depth + rand normal, 2: rand depth + cur normal
-        const float hd = (hsel == 1) ? kd : rd;
-        const float hn0 = (hsel == 2) ? kn0 : rn0, hn1 = (hsel == 2) ? kn1 : rn1, hn2 = (hsel == 2) ? kn2 : rn2;
-        const PmSrcDesc sd = P.src[img];
-        const float c = pm_ncc_group<3, 3, 1>(kwr, off, P.ntaps, poses + img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off, sd.pitch,
-                                              sd.w, sd.h, krow, kcol, hd, hn0, hn1, hn2, kiw, krs, krq, sub, gmask, ph);
-        if (sub == 0) A.tab3[(kp * 3 + hsel) * N + img] = c;
-        ph(PM_PH_FINAL);
-        return c;
-      };
-      if (!PRUNE) {   // every (hypothesis, image) pair, four per round
-        const int npairs = 3 * N;
-        for (int base = 0; base < npairs; base += 4) {
-          const int pair = base + g;
-          ph(PM_PH_SELECT);
-          if (pair < npairs) ncc(pair / N, pair % N);
-        }
-        continue;
-      }
-      const int kmult = __shfl_sync(full, mult, src);   // lanes 0..7: multiplicity of image lane
-      const float kthr = __shfl_sync(full, thr, 8 * k);
-      const float kgc = GEOM ? __shfl_sync(full, gcur, src) : 0.0f, kgr = GEOM ? __shfl_sync(full, grand, src) : 0.0f;
-      const unsigned needed = (needed4 >> (8 * k)) & 0xffu;
-      unsigned rem0 = nmask, rem1 = nmask, rem2 = nmask, ev0 = 0u, ev1 = 0u, ev2 = 0u;
-      bool act0 = true, act1 = true, act2 = true, ext0 = true, ext1 = true, ext2 = true;
-      if (mode == 1) {
-        rem0 = rem1 = rem2 = needed;
-        ext0 = ext1 = ext2 = false;
-        act0 = act1 = act2 = needed != 0u;
-      } else if (mode != 0) {
-        act0 = act1 = act2 = false;
-      }
-      float L0 = 0.0f, L1 = 0.0f, L2 = 0.0f;
-      while (act0 || act1 || act2) {
-        // up to four (hypothesis, image) pairs per round, hypotheses taking turns, images by multiplicity
-        int my_k = -1, my_img = 0, slot = 0;
+    // ---- pooled rounds.  Segment k (lanes 8k..8k+7) carries pixel k's round state, warp-uniform within the segment:
+    // per hypothesis h (0: rand/rand, 1: cur depth + rand normal, 2: rand depth + cur normal) the images left (rem) and
+    // the images evaluated (ev), byte h of each, a bit per image RANK: rank r is image (ord >> 4r) & 15, the images
+    // sorted by multiplicity, then by index (the order in which a hypothesis takes its images; the images nobody
+    // sampled come last, and lanes >= N after them).  Unpruned (mode 0), every image of every hypothesis is left and
+    // nothing is ever dropped.
+    const unsigned key = (((unsigned)mult << 5) | (unsigned)(31 - sub)) + 1u;
+    int rank = 0;
 #pragma unroll
-        for (int pass = 0; pass < 2; ++pass) {
+    for (int j = 0; j < 8; ++j) rank += (__shfl_sync(full, key, j, 8) > key) ? 1 : 0;
+    unsigned ord = (unsigned)sub << (4 * rank);
 #pragma unroll
-          for (int h = 0; h < 3; ++h) {
-            const bool a = (h == 0) ? act0 : ((h == 1) ? act1 : act2);
-            const unsigned rem = (h == 0) ? rem0 : ((h == 1) ? rem1 : rem2);
-            if (slot < 4 && a && rem) {
-              const unsigned key = ((rem >> lane) & 1u) ? ((((unsigned)kmult) << 5) | (unsigned)(31 - lane)) + 1u : 0u;
-              const unsigned best = __reduce_max_sync(full, key);
-              const int im = 31 - (int)((best - 1u) & 31u);
-              const unsigned bit = 1u << im;
-              if (h == 0) { rem0 &= ~bit; ev0 |= bit; } else if (h == 1) { rem1 &= ~bit; ev1 |= bit; } else { rem2 &= ~bit; ev2 |= bit; }
-              if (slot == g) { my_k = h; my_img = im; }
-              ++slot;
-            }
-          }
+    for (int o = 1; o < 8; o <<= 1) ord |= __shfl_xor_sync(full, ord, o, 8);
+    unsigned rem = nmask * 0x10101u, ev = 0u, act = live ? 7u : 0u, ext = 7u;   // act / ext: bit h
+    if (PRUNE) {
+      const unsigned need = (1u << __popc((needed4 >> (8 * g)) & 0xffu)) - 1u;   // the sampled images: the first ranks
+      rem = need * 0x10101u;
+      ext = 0u;
+      act = (mode == 1 && need) ? 7u : 0u;
+    }
+    float L0 = 0.0f, L1 = 0.0f, L2 = 0.0f;
+    unsigned hp = 0u;   // the hypothesis whose turn is next
+    for (;;) {
+      // Fill the four group slots in passes: in each pass every pixel with a pair left proposes one, its next
+      // hypothesis in turn and that hypothesis' first image left, and pixel by pixel the proposals take the free slots.
+      // A pixel left alone takes all four slots in four passes.  Group g evaluates the pair of slot g.
+      int my_code = -1, slot = 0;   // my_code: pixel << 8 | h << 4 | image
+      for (int pass = 0; pass < 4 && slot < 4; ++pass) {
+        const unsigned avail = act & (((rem & 0xffu) ? 1u : 0u) | ((rem & 0xff00u) ? 2u : 0u) | ((rem & 0xff0000u) ? 4u : 0u));
+        const unsigned turn = ((avail | (avail << 3)) >> hp) & 7u;
+        unsigned h = hp + (unsigned)__ffs(turn) - 1u;
+        if (h >= 3u) h -= 3u;
+        const unsigned rbit = ((rem >> (8 * h)) & 0xffu) & (0u - ((rem >> (8 * h)) & 0xffu));   // lowest rank left
+        const int img = (int)((ord >> (4 * (__ffs(rbit) - 1))) & 15u);
+        const unsigned b = __ballot_sync(full, turn != 0u);
+        const unsigned pm = (b & 1u) | ((b >> 7) & 2u) | ((b >> 14) & 4u) | ((b >> 21) & 8u);   // pixels proposing
+        if (!pm) break;
+        if (turn && slot + __popc(pm & ((1u << g) - 1u)) < 4) {   // this pixel's proposal got a slot
+          rem &= ~(rbit << (8 * h));
+          ev |= rbit << (8 * h);
+          hp = (h == 2u) ? 0u : h + 1u;
         }
+        const int j = g - slot;   // this group's slot takes the proposal of the j-th proposing pixel, if there is one
+        int src = g;
+#pragma unroll
+        for (int kk = 3; kk >= 0; --kk)
+          if (((pm >> kk) & 1u) && __popc(pm & ((1u << kk) - 1u)) == j) src = kk;
+        const int code = (g << 8) | (int)(h << 4) | img;
+        const int got = __shfl_sync(full, code, 8 * src);
+        if (j >= 0 && j < __popc(pm)) my_code = got;
+        slot = min(4, slot + __popc(pm));
+      }
+      ph(PM_PH_SELECT);
+      if (slot == 0) break;
+      PM_POOL_COUNT(n_rounds, 1);
+      PM_POOL_COUNT(n_ncc, slot);
+      // pixel kk's values, from the lanes of segment kk
+      const int kk = my_code < 0 ? g : (my_code >> 8), my_h = (my_code >> 4) & 15, my_img = my_code & 15;
+      const float krow = __shfl_sync(full, rowf, 8 * kk), kcol = __shfl_sync(full, colf, 8 * kk);
+      const float kd = __shfl_sync(full, cur_d, 8 * kk), kn0 = __shfl_sync(full, cn0, 8 * kk), kn1 = __shfl_sync(full, cn1, 8 * kk),
+                  kn2 = __shfl_sync(full, cn2, 8 * kk);
+      const float rd = __shfl_sync(full, r4.x, 8 * kk), rn0 = __shfl_sync(full, r4.y, 8 * kk), rn1 = __shfl_sync(full, r4.z, 8 * kk),
+                  rn2 = __shfl_sync(full, r4.w, 8 * kk);
+      const float kiw = __shfl_sync(full, inv_wsum, 8 * kk), krs = __shfl_sync(full, rsum, 8 * kk), krq = __shfl_sync(full, rsq, 8 * kk);
+      float c = 0.0f;
+      if (my_code >= 0) {
+        const float hd = (my_h == 1) ? kd : rd;
+        const float hn0 = (my_h == 2) ? kn0 : rn0, hn1 = (my_h == 2) ? kn1 : rn1, hn2 = (my_h == 2) ? kn2 : rn2;
+        const PmSrcDesc sd = P.src[my_img];
         ph(PM_PH_SELECT);
-        if (slot == 0) break;
-        float c = 0.0f;
-        if (my_k >= 0) c = ncc(my_k, my_img);
-        if (mode == 1) {
-#pragma unroll
-          for (int s2 = 0; s2 < 4; ++s2) {
-            const int ks = __shfl_sync(full, my_k, 8 * s2), is = __shfl_sync(full, my_img, 8 * s2);
-            float v = __shfl_sync(full, c, 8 * s2);
-            const float w = (float)__shfl_sync(full, kmult, is & 31);
-            if (GEOM) v = fmaf(P.geom_reg, __shfl_sync(full, (ks == 1) ? kgc : kgr, is & 31), v);
-            if (ks == 0) L0 = fmaf(w, v, L0); else if (ks == 1) L1 = fmaf(w, v, L1); else if (ks == 2) L2 = fmaf(w, v, L2);
-          }
-          // a hypothesis whose partial sum already exceeds the current hypothesis' sum is out; one that survives all its
-          // sampled images is a likely winner: the images nobody sampled are then needed for the cost map (:1184-1196)
-          if (act0) { if (L0 > kthr) act0 = false; else if (!rem0) { if (!ext0) { ext0 = true; rem0 = nmask & ~ev0; } if (!rem0) act0 = false; } }
-          if (act1) { if (L1 > kthr) act1 = false; else if (!rem1) { if (!ext1) { ext1 = true; rem1 = nmask & ~ev1; } if (!rem1) act1 = false; } }
-          if (act2) { if (L2 > kthr) act2 = false; else if (!rem2) { if (!ext2) { ext2 = true; rem2 = nmask & ~ev2; } if (!rem2) act2 = false; } }
-        } else {
-          act0 = rem0 != 0u; act1 = rem1 != 0u; act2 = rem2 != 0u;
-        }
-        ph(PM_PH_BOUND);
+        c = pm_ncc_group<3, 3, 1>(wr_warp + kk * tp, off, P.ntaps, poses + my_img * PM_POSE_STRIDE, iK, P.quads + sd.quad_off,
+                                  sd.pitch, sd.w, sd.h, krow, kcol, hd, hn0, hn1, hn2, kiw, krs, krq, sub, gmask, ph);
+        const size_t kp = pm_pix0(P.W0, P.H0, rot, (int)krow, (int)kcol);
+        if (sub == 0) A.tab3[(kp * 3 + my_h) * N + my_img] = c;
+        ph(PM_PH_FINAL);
       }
+      if (PRUNE) {
+        // each segment adds its pixel's results of the round, in slot order
+#pragma unroll
+        for (int s2 = 0; s2 < 4; ++s2) {
+          const int cs = __shfl_sync(full, my_code, 8 * s2);
+          float v = __shfl_sync(full, c, 8 * s2);
+          const int hs = (cs >> 4) & 15, is = cs & 7;
+          const float w = (float)__shfl_sync(full, mult, 8 * g + is);
+          if (GEOM) v = fmaf(P.geom_reg, __shfl_sync(full, (hs == 1) ? gcur : grand, 8 * g + is), v);
+          if (cs >= 0 && (cs >> 8) == g) {
+            if (hs == 0) L0 = fmaf(w, v, L0); else if (hs == 1) L1 = fmaf(w, v, L1); else L2 = fmaf(w, v, L2);
+          }
+        }
+      }
+      // a hypothesis whose partial sum already exceeds the current hypothesis' sum is out; one that survives all its
+      // sampled images is a likely winner: the images nobody sampled are then needed for the cost map (:1184-1196)
+#pragma unroll
+      for (int h = 0; h < 3; ++h) {
+        const float Lh = (h == 0) ? L0 : ((h == 1) ? L1 : L2);
+        if ((act >> h) & 1u) {
+          if (Lh > thr) {
+            act &= ~(1u << h);
+          } else if (!((rem >> (8 * h)) & 0xffu)) {
+            if (!((ext >> h) & 1u)) { ext |= 1u << h; rem |= (nmask & ~(ev >> (8 * h))) << (8 * h); }
+            if (!((rem >> (8 * h)) & 0xffu)) act &= ~(1u << h);
+          }
+        }
+      }
+      ph(PM_PH_BOUND);
     }
     __syncwarp();   // every group is done with the batch's patches before the next batch's copies overwrite them
   }
 #ifdef PM_PIXEL_PHASES
-  if (lane == 0)
+  if (lane == 0) {
     for (int k = 0; k < PM_PH_COUNT; ++k) atomicAdd(&pm_phase_cycles[PRUNE ? 1 : 0][k], ph_acc[warp][k]);
+    atomicAdd(&pm_pool_counts[PRUNE ? 1 : 0][PM_CNT_P_NCC], n_ncc);
+    atomicAdd(&pm_pool_counts[PRUNE ? 1 : 0][PM_CNT_P_ROUNDS], n_rounds);
+  }
 #endif
 }
 
@@ -1193,6 +1223,9 @@ __global__ void __launch_bounds__(32 * WPC, 16 / WPC) pm_serial_kernel(const PmP
       auto evaluate = [&](int k, unsigned todo) {
         const float hd = (k == 3) ? cur_d : r4.x;
         const float hn0 = (k == 4) ? cur_n0 : r4.y, hn1 = (k == 4) ? cur_n1 : r4.z, hn2 = (k == 4) ? cur_n2 : r4.w;
+#ifdef PM_PIXEL_PHASES
+        if (lane == 0) atomicAdd(&pm_pool_counts[A.prune ? 1 : 0][PM_CNT_S_NCC], (unsigned long long)__popc(todo));
+#endif
         while (todo) {
           int my_img = -1;
 #pragma unroll
@@ -1947,6 +1980,16 @@ int b200pm_debug_get_cost(b200pm_handle c, float* cost) {
   return 0;
 }
 
+// debug: the last sweep's tab3 ([pixel][3][N], pixel in the original orientation), PM_NOT_EVALUATED where the pixel
+// pass left an entry out
+int b200pm_debug_get_tab3(b200pm_handle c, float* out) {
+  if (!c) return pm_fail(-1, "null handle");
+  PM_CUDA(cudaSetDevice(c->device));
+  const size_t n = (size_t)c->P.W0 * c->P.H0;
+  PM_CUDA(cudaMemcpy(out, c->tab3, sizeof(float) * 3 * n * c->P.N, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
 // ---- host-side hooks for the CPU test tier (bit-level comparison with the oracle; no GPU needed) ----
 float b200pm_test_expf(float x) { return pm_expf(x); }
 void b200pm_test_sincosf(float a, float* s, float* c) { pm_sincosf(a, s, c); }
@@ -1987,6 +2030,14 @@ int b200pm_debug_pixel_phases(unsigned long long* out) {
   const unsigned long long zero[2][PM_PH_COUNT] = {};
   PM_CUDA(cudaMemcpyToSymbol(pm_phase_cycles, zero, sizeof(zero)));
   return PM_PH_COUNT;
+}
+// diagnostic build: out[pruned * PM_CNT_COUNT + k] = pm_pool_counts since the last call, then reset
+int b200pm_debug_pool_counts(unsigned long long* out) {
+  PM_CUDA(cudaDeviceSynchronize());
+  PM_CUDA(cudaMemcpyFromSymbol(out, pm_pool_counts, sizeof(pm_pool_counts)));
+  const unsigned long long zero[2][PM_CNT_COUNT] = {};
+  PM_CUDA(cudaMemcpyToSymbol(pm_pool_counts, zero, sizeof(zero)));
+  return PM_CNT_COUNT;
 }
 #endif
 
