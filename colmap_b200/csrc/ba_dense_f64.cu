@@ -282,3 +282,13 @@ cudaError_t ba_dense_potrs(const double* A, int N, const double* dinv, int nrhs,
     ba_trsv_bwd<<<dim3(ba_blocks((long long)k * T, TB / 32), nrhs), TB, 0, st>>>(A, dinv, N, k, W, B, flag);
   return cudaGetLastError();
 }
+
+__global__ void ba_pad_identity_kernel(double* A, int n, int N) {
+  const int i = n + blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < N) A[(long long)i * N + i] = 1.0;
+}
+
+cudaError_t ba_dense_pad_identity(double* A, int N, int n, cudaStream_t st) {
+  if (N > n) ba_pad_identity_kernel<<<ba_blocks(N - n, 64), 64, 0, st>>>(A, n, N);
+  return cudaGetLastError();
+}

@@ -20,6 +20,8 @@ struct BaDenseFlag {
   double pivot;   // its value
 };
 
+// A(i, i) = 1 for n <= i < N: the identity block of the padding (the caller zeroes A first).  Launches nothing when N == n.
+cudaError_t ba_dense_pad_identity(double* A, int N, int n, cudaStream_t st);
 // A = L L^T in place (lower triangle).  The pivot of row r fails when !(d > pivot_min) for n_test0 <= r < n_check
 // (the rank test), when !(d > 0) for r < n_test0 (positive definiteness only), and is not tested for r >= n_check
 // (padding).  dinv: [N * BA_TILE] scratch that receives the inverse of every diagonal tile of L (read again by

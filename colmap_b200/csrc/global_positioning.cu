@@ -16,8 +16,6 @@
 #include <cuda_runtime.h>
 #include <float.h>
 #include <math.h>
-#include <stdarg.h>
-#include <stdio.h>
 #include <string.h>
 
 #include <algorithm>
@@ -27,14 +25,10 @@
 #include "../../include/b200_global_positioning.h"
 #include "ba_dense_f64.h"
 #include "ba_models.cuh"
+#include "solver_host.cuh"
 
 static thread_local std::string g_gp_err;
-static int gp_fail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof buf, fmt, ap); va_end(ap);
-  g_gp_err = buf;
-  return code;
-}
+#define GP_CHECK(call) SOLVER_CUDA(g_gp_err, B200GP_ERR_CUDA, call)
 extern "C" const char* b200gp_last_error(void) { return g_gp_err.c_str(); }
 
 extern "C" void b200gp_options_init(b200gp_options* o) {
@@ -170,7 +164,7 @@ static bool gp_cam_from_img(int id, const double* p, double x, double y, double*
 }
 
 extern "C" int b200gp_cam_ray_from_img(int model_id, const double* params, const double* xy, double* ray) {
-  if (model_id < 0 || model_id > 17 || !params || !xy || !ray) return gp_fail(B200GP_ERR_INPUT, "cam_ray_from_img: bad arguments");
+  if (model_id < 0 || model_id > 17 || !params || !xy || !ray) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "cam_ray_from_img: bad arguments");
   if (model_id == 17) {   // EquirectangularCameraModel::CamRayFromImg (models.h:809-829)
     const double theta = 2.0 * M_PI * (xy[0] / params[0] - 0.5), phi = M_PI * (0.5 - xy[1] / params[1]);
     const double cp = cos(phi);
@@ -178,7 +172,7 @@ extern "C" int b200gp_cam_ray_from_img(int model_id, const double* params, const
     return 0;
   }
   double u = 0, v = 0;
-  if (!gp_cam_from_img(model_id, params, xy[0], xy[1], &u, &v)) return gp_fail(B200GP_ERR_INPUT, "cam_ray_from_img: not unprojectable");
+  if (!gp_cam_from_img(model_id, params, xy[0], xy[1], &u, &v)) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "cam_ray_from_img: not unprojectable");
   const double n = sqrt(u * u + v * v + 1.0);
   ray[0] = u / n; ray[1] = v / n; ray[2] = 1.0 / n;
   return 0;
@@ -418,11 +412,6 @@ __global__ void k_rows(GpDev g, double radius, double dmin, double dmax, const u
   g.rhs[i] = rhs;
 }
 
-__global__ void k_pad_identity(double* A, int n, int Npad) {
-  const int i = n + blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < Npad) A[(int64_t)i * Npad + i] = 1.0;
-}
-
 // back-substitution to the points: dX = H^-1 (-g_p - sum E dC)
 __global__ void k_back_points(GpDev g) {
   const int64_t vp = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -477,266 +466,259 @@ __global__ void k_update_blocks(GpDev g, const uint8_t* pvar) {
   if (i < 3 * g.P) { const int64_t p = i / 3; g.X2[i] = pvar[p] ? g.X[i] + g.Dp[i] * g.dX[i] : g.X[i]; }
 }
 
-// deterministic sums: fixed grid, fixed per-thread order, fixed tree
-#define GP_RB 256
-#define GP_RG 512
-// mode 0: sum a; 1: sum (a - b)^2 over mask; 2: sum a^2 over mask
-__global__ void k_reduce1(const double* a, const double* b, const uint8_t* mask, int mstride, int64_t n, int mode, double* part) {
-  __shared__ double sh[GP_RB];
-  double s = 0;
-  for (int64_t i = blockIdx.x * (int64_t)GP_RB + threadIdx.x; i < n; i += (int64_t)GP_RG * GP_RB) {
-    if (mode && mask && !mask[i / mstride]) continue;
-    const double v = mode == 1 ? a[i] - b[i] : a[i];
-    s += mode ? v * v : v;
-  }
-  sh[threadIdx.x] = s;
-  __syncthreads();
-  for (int o = GP_RB / 2; o; o >>= 1) { if (threadIdx.x < o) sh[threadIdx.x] += sh[threadIdx.x + o]; __syncthreads(); }
-  if (!threadIdx.x) part[blockIdx.x] = sh[0];
-}
-__global__ void k_reduce2(double* part, double* out) {
-  __shared__ double sh[GP_RG];
-  for (int i = threadIdx.x; i < GP_RG; i += GP_RB) sh[i] = part[i];
-  __syncthreads();
-  for (int o = GP_RG / 2; o; o >>= 1) { for (int i = threadIdx.x; i < o; i += GP_RB) sh[i] += sh[i + o]; __syncthreads(); }
-  if (!threadIdx.x) *out = sh[0];
-}
 
 // ------------------------------------------------------------------------------------------------ host
-#define GP_CUDA(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { rc = gp_fail(B200GP_ERR_CUDA, "%s: %s", #x, cudaGetErrorString(e_)); goto cleanup; } } while (0)
+#define GP_RG 512   // CTAs of the deterministic sums
 
-static inline unsigned gp_blocks(int64_t n, int t) { return (unsigned)std::max<int64_t>(1, (n + t - 1) / t); }
-
-static bool finite_all(const double* a, int64_t n) { for (int64_t i = 0; i < n; ++i) if (!std::isfinite(a[i])) return false; return true; }
-
-extern "C" int b200gp_solve(const b200gp_options* o, b200gp_problem* p, b200gp_summary* out) {
-  g_gp_err.clear();
-  if (!o || !p || !out) return gp_fail(B200GP_ERR_INPUT, "null argument");
-  // ---- options
-  if (!(o->loss_function_scale > 0) || !std::isfinite(o->loss_function_scale)) return gp_fail(B200GP_ERR_INPUT, "loss_function_scale must be positive");
+// options and problem checks, host only
+static int gp_check(const b200gp_options* o, const b200gp_problem* p) {
+  if (!(o->loss_function_scale > 0) || !std::isfinite(o->loss_function_scale)) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "loss_function_scale must be positive");
   if (o->max_num_iterations < 0 || !(o->function_tolerance >= 0) || !(o->gradient_tolerance >= 0) || !(o->parameter_tolerance >= 0) ||
       !(o->initial_trust_region_radius > 0) || !(o->max_trust_region_radius >= o->initial_trust_region_radius) ||
       !(o->min_trust_region_radius >= 0) || !(o->min_lm_diagonal > 0) || !(o->max_lm_diagonal >= o->min_lm_diagonal) ||
       !(o->min_relative_decrease >= 0))
-    return gp_fail(B200GP_ERR_INPUT, "invalid solver options");
+    return solver_fail(g_gp_err, B200GP_ERR_INPUT, "invalid solver options");
   const int F = p->num_frames, S = p->num_sensors; const int64_t P = p->num_points, N = p->num_observations;
-  if (F < 0 || S < 0 || P < 0 || N < 0) return gp_fail(B200GP_ERR_INPUT, "negative size");
+  if (F < 0 || S < 0 || P < 0 || N < 0) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "negative size");
   if ((F && !p->frame_centers) || (P && !p->points) || (S && !p->cams_in_rig) ||
       (N && (!p->obs_frame || !p->obs_point || !p->obs_ray || !p->obs_scale)))
-    return gp_fail(B200GP_ERR_INPUT, "missing array");
-  if (!finite_all(p->frame_centers, 3LL * F)) return gp_fail(B200GP_ERR_INPUT, "non-finite frame centre");
-  if (!finite_all(p->points, 3 * P)) return gp_fail(B200GP_ERR_INPUT, "non-finite point");
-  if (!finite_all(p->cams_in_rig, 3LL * S)) return gp_fail(B200GP_ERR_INPUT, "non-finite camera-in-rig position");
-  if (!finite_all(p->obs_ray, 3 * N)) return gp_fail(B200GP_ERR_INPUT, "non-finite ray");
-  if (p->obs_rig_offset && !finite_all(p->obs_rig_offset, 3 * N)) return gp_fail(B200GP_ERR_INPUT, "non-finite rig offset");
-  std::vector<uint8_t> frame_used(F, 0), sensor_used(S, 0), point_used(P, 0);
+    return solver_fail(g_gp_err, B200GP_ERR_INPUT, "missing array");
+  if (!all_finite(p->frame_centers, 3LL * F)) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "non-finite frame centre");
+  if (!all_finite(p->points, 3 * P)) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "non-finite point");
+  if (!all_finite(p->cams_in_rig, 3LL * S)) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "non-finite camera-in-rig position");
+  if (!all_finite(p->obs_ray, 3 * N)) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "non-finite ray");
+  if (p->obs_rig_offset && !all_finite(p->obs_rig_offset, 3 * N)) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "non-finite rig offset");
   for (int64_t j = 0; j < N; ++j) {
     const int f = p->obs_frame[j]; const int64_t q = p->obs_point[j]; const int s = p->obs_sensor ? p->obs_sensor[j] : -1;
-    if (f < 0 || f >= F) return gp_fail(B200GP_ERR_INPUT, "observation %lld: frame %d out of range", (long long)j, f);
-    if (q < 0 || q >= P) return gp_fail(B200GP_ERR_INPUT, "observation %lld: point %lld out of range", (long long)j, (long long)q);
-    if (s < -1 || s >= S) return gp_fail(B200GP_ERR_INPUT, "observation %lld: sensor %d out of range", (long long)j, s);
+    if (f < 0 || f >= F) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "observation %lld: frame %d out of range", (long long)j, f);
+    if (q < 0 || q >= P) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "observation %lld: point %lld out of range", (long long)j, (long long)q);
+    if (s < -1 || s >= S) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "observation %lld: sensor %d out of range", (long long)j, s);
     if (s >= 0 && !o->refine_sensor_from_rig)
-      return gp_fail(B200GP_ERR_INPUT, "observation %lld: variable camera-in-rig position but refine_sensor_from_rig = 0", (long long)j);
-    if (s >= 0 && !p->world_from_rig) return gp_fail(B200GP_ERR_INPUT, "world_from_rig is needed for sensor observations");
-    if (s >= 0 && !finite_all(p->world_from_rig + 9LL * f, 9)) return gp_fail(B200GP_ERR_INPUT, "non-finite world_from_rig of frame %d", f);
+      return solver_fail(g_gp_err, B200GP_ERR_INPUT, "observation %lld: variable camera-in-rig position but refine_sensor_from_rig = 0", (long long)j);
+    if (s >= 0 && !p->world_from_rig) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "world_from_rig is needed for sensor observations");
+    if (s >= 0 && !all_finite(p->world_from_rig + 9LL * f, 9)) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "non-finite world_from_rig of frame %d", f);
     const double sc = p->obs_scale[j];
-    if (!std::isfinite(sc) || sc < B200GP_SCALE_LOWER_BOUND) return gp_fail(B200GP_ERR_INPUT, "observation %lld: scale %g below the bound 1e-5 or not finite", (long long)j, sc);
+    if (!std::isfinite(sc) || sc < B200GP_SCALE_LOWER_BOUND) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "observation %lld: scale %g below the bound 1e-5 or not finite", (long long)j, sc);
     const double w = p->obs_loss_weight ? p->obs_loss_weight[j] : 1.0;
-    if (!(w > 0) || !std::isfinite(w)) return gp_fail(B200GP_ERR_INPUT, "observation %lld: loss weight must be positive", (long long)j);
-    frame_used[f] = 1; point_used[q] = 1; if (s >= 0) sensor_used[s] = 1;
+    if (!(w > 0) || !std::isfinite(w)) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "observation %lld: loss weight must be positive", (long long)j);
+  }
+  return 0;
+}
+
+// The device layout of a checked problem: variable blocks, and the observations sorted by point with the per-point
+// ranges and the block -> (observation, slot) lists of GpDev.
+struct GpLayout {
+  int nb, n, Npad;
+  int64_t nvp;
+  std::vector<int> fblk, sblk, blk_frame, blk_sensor;   // frame / sensor -> block (-1: constant), block -> frame / sensor
+  std::vector<uint8_t> pvar, fmask, sensor_used;        // variable points, variable frames, variable sensors
+  std::vector<int64_t> perm;                            // sorted position -> caller's observation
+  std::vector<double> ray, off, R, w, s;
+  std::vector<int> fr, sen, blk;
+  std::vector<int64_t> pt, vp_start, vp_pt, obs_vp, bl_start, bl_ent;
+  std::vector<uint8_t> svar;
+};
+
+static int gp_layout(const b200gp_options* o, const b200gp_problem* p, GpLayout& L) {
+  const int F = p->num_frames, S = p->num_sensors; const int64_t P = p->num_points, N = p->num_observations;
+  std::vector<uint8_t> frame_used(F, 0), point_used(P, 0);
+  L.sensor_used.assign(S, 0);
+  for (int64_t j = 0; j < N; ++j) {
+    frame_used[p->obs_frame[j]] = 1; point_used[p->obs_point[j]] = 1;
+    if (p->obs_sensor && p->obs_sensor[j] >= 0) L.sensor_used[p->obs_sensor[j]] = 1;
   }
   // ---- variable blocks
-  std::vector<int> fblk(F, -1), sblk(S, -1), blk_frame, blk_sensor;
+  L.fblk.assign(F, -1); L.sblk.assign(S, -1);
   for (int f = 0; f < F; ++f)
-    if (frame_used[f] && o->optimize_positions && !(p->frame_constant && p->frame_constant[f])) { fblk[f] = (int)blk_frame.size(); blk_frame.push_back(f); blk_sensor.push_back(-1); }
+    if (frame_used[f] && o->optimize_positions && !(p->frame_constant && p->frame_constant[f])) { L.fblk[f] = (int)L.blk_frame.size(); L.blk_frame.push_back(f); L.blk_sensor.push_back(-1); }
   for (int s = 0; s < S; ++s)
-    if (sensor_used[s]) { sblk[s] = (int)blk_frame.size(); blk_frame.push_back(-1); blk_sensor.push_back(s); }
-  const int nb = (int)blk_frame.size();
+    if (L.sensor_used[s]) { L.sblk[s] = (int)L.blk_frame.size(); L.blk_frame.push_back(-1); L.blk_sensor.push_back(s); }
+  const int nb = (int)L.blk_frame.size();
   if (3LL * nb > B200GP_MAX_REDUCED_DIM)
-    return gp_fail(B200GP_ERR_TOO_LARGE, "reduced dimension %lld exceeds the dense limit %d (a sparse reduced solve is not implemented)", 3LL * nb, B200GP_MAX_REDUCED_DIM);
-  const int n = 3 * nb, Npad = (n + BA_TILE - 1) / BA_TILE * BA_TILE;
-  std::vector<uint8_t> pvar(P, 0);
-  for (int64_t q = 0; q < P; ++q) pvar[q] = point_used[q] && o->optimize_points;
+    return solver_fail(g_gp_err, B200GP_ERR_TOO_LARGE, "reduced dimension %lld exceeds the dense limit %d (a sparse reduced solve is not implemented)", 3LL * nb, B200GP_MAX_REDUCED_DIM);
+  L.nb = nb; L.n = 3 * nb; L.Npad = (L.n + BA_TILE - 1) / BA_TILE * BA_TILE;
+  L.pvar.assign(P, 0);
+  for (int64_t q = 0; q < P; ++q) L.pvar[q] = point_used[q] && o->optimize_points;
+  L.fmask.assign(F, 0);
+  for (int f = 0; f < F; ++f) L.fmask[f] = L.fblk[f] >= 0;
   // ---- sort observations by point (stable)
-  std::vector<int64_t> perm(N);
-  for (int64_t j = 0; j < N; ++j) perm[j] = j;
-  std::stable_sort(perm.begin(), perm.end(), [&](int64_t a, int64_t b) { return p->obs_point[a] < p->obs_point[b]; });
-  std::vector<double> h_ray(3 * N), h_off(3 * N, 0.0), h_R(9 * N, 0.0), h_w(N), h_s(N);
-  std::vector<int> h_fr(N), h_sen(N), h_blk(2 * N);
-  std::vector<int64_t> h_pt(N), vp_start, vp_pt;
-  std::vector<uint8_t> h_svar(N);
-  std::vector<int64_t> bl_count(nb + 1, 0);
+  L.perm.resize(N);
+  for (int64_t j = 0; j < N; ++j) L.perm[j] = j;
+  std::stable_sort(L.perm.begin(), L.perm.end(), [&](int64_t a, int64_t b) { return p->obs_point[a] < p->obs_point[b]; });
+  L.ray.resize(3 * N); L.off.assign(3 * N, 0.0); L.R.assign(9 * N, 0.0); L.w.resize(N); L.s.resize(N);
+  L.fr.resize(N); L.sen.resize(N); L.blk.resize(2 * N); L.pt.resize(N); L.svar.resize(N);
+  L.bl_start.assign(nb + 1, 0);
+  std::vector<int64_t> vp_first;
   for (int64_t j = 0; j < N; ++j) {
-    const int64_t o_ = perm[j];
+    const int64_t o_ = L.perm[j];
     const int f = p->obs_frame[o_], s = p->obs_sensor ? p->obs_sensor[o_] : -1;
-    for (int m = 0; m < 3; ++m) { h_ray[3 * j + m] = p->obs_ray[3 * o_ + m]; if (s < 0 && p->obs_rig_offset) h_off[3 * j + m] = p->obs_rig_offset[3 * o_ + m]; }
-    if (s >= 0) for (int m = 0; m < 9; ++m) h_R[9 * j + m] = p->world_from_rig[9LL * f + m];
-    h_w[j] = p->obs_loss_weight ? p->obs_loss_weight[o_] : 1.0;
-    h_s[j] = p->obs_scale[o_];
-    h_fr[j] = f; h_sen[j] = s; h_pt[j] = p->obs_point[o_];
-    h_blk[2 * j] = fblk[f]; h_blk[2 * j + 1] = s >= 0 ? sblk[s] : -1;
-    h_svar[j] = o->optimize_scales && o_ != 0;
-    for (int k = 0; k < 2; ++k) if (h_blk[2 * j + k] >= 0) bl_count[h_blk[2 * j + k] + 1]++;
-    if (pvar[h_pt[j]] && (j == 0 || h_pt[j - 1] != h_pt[j])) { vp_start.push_back(j); vp_pt.push_back(h_pt[j]); }
+    for (int m = 0; m < 3; ++m) { L.ray[3 * j + m] = p->obs_ray[3 * o_ + m]; if (s < 0 && p->obs_rig_offset) L.off[3 * j + m] = p->obs_rig_offset[3 * o_ + m]; }
+    if (s >= 0) for (int m = 0; m < 9; ++m) L.R[9 * j + m] = p->world_from_rig[9LL * f + m];
+    L.w[j] = p->obs_loss_weight ? p->obs_loss_weight[o_] : 1.0;
+    L.s[j] = p->obs_scale[o_];
+    L.fr[j] = f; L.sen[j] = s; L.pt[j] = p->obs_point[o_];
+    L.blk[2 * j] = L.fblk[f]; L.blk[2 * j + 1] = s >= 0 ? L.sblk[s] : -1;
+    L.svar[j] = o->optimize_scales && o_ != 0;
+    for (int k = 0; k < 2; ++k) if (L.blk[2 * j + k] >= 0) L.bl_start[L.blk[2 * j + k] + 1]++;
+    if (L.pvar[L.pt[j]] && (j == 0 || L.pt[j - 1] != L.pt[j])) { vp_first.push_back(j); L.vp_pt.push_back(L.pt[j]); }
   }
-  const int64_t nvp = (int64_t)vp_pt.size();
-  {   // [start, end) per variable point: a point's observations are contiguous in the sorted order
-    std::vector<int64_t> ranges(std::max<int64_t>(1, 2 * nvp));
-    for (int64_t k = 0; k < nvp; ++k) {
-      int64_t e = vp_start[k];
-      while (e < N && h_pt[e] == vp_pt[k]) ++e;
-      ranges[2 * k] = vp_start[k]; ranges[2 * k + 1] = e;
+  const int64_t nvp = (int64_t)L.vp_pt.size();
+  L.nvp = nvp;
+  // [start, end) per variable point: a point's observations are contiguous in the sorted order
+  L.vp_start.assign(std::max<int64_t>(1, 2 * nvp), 0);
+  for (int64_t k = 0; k < nvp; ++k) {
+    int64_t e = vp_first[k];
+    while (e < N && L.pt[e] == L.vp_pt[k]) ++e;
+    L.vp_start[2 * k] = vp_first[k]; L.vp_start[2 * k + 1] = e;
+  }
+  L.obs_vp.assign(N, -1);
+  for (int64_t k = 0; k < nvp; ++k) for (int64_t j = L.vp_start[2 * k]; j < L.vp_start[2 * k + 1]; ++j) L.obs_vp[j] = k;
+  for (int b = 0; b < nb; ++b) L.bl_start[b + 1] += L.bl_start[b];
+  L.bl_ent.assign(std::max<int64_t>(1, L.bl_start[nb]), 0);
+  std::vector<int64_t> fill(L.bl_start.begin(), L.bl_start.end() - 1);
+  for (int64_t j = 0; j < N; ++j) for (int k = 0; k < 2; ++k) { const int b = L.blk[2 * j + k]; if (b >= 0) L.bl_ent[fill[b]++] = 2 * j + k; }
+  return 0;
+}
+
+// The LM solve (Levenberg-Marquardt with Ceres' trust-region rules) on the device state g.  Every method returns 0 or
+// B200GP_ERR_CUDA.
+struct GpSolve {
+  const b200gp_options* o;
+  b200gp_summary* out;
+  GpDev g;
+  uint8_t *pvar, *fmask, *qmask, *smask;   // variable points, frames, sensors and scales
+
+  // deterministic sum of cnt terms (solver_sum mode) into *r
+  int dsum(int mode, const double* x, const double* y, const uint8_t* mask, int stride, int64_t cnt, double* r) {
+    *r = 0.0;
+    if (cnt <= 0) return 0;
+    solver_sum<GP_RG>(mode, x, y, mask, stride, cnt, g.red, g.red + GP_RG);
+    GP_CHECK(cudaMemcpy(r, g.red + GP_RG, sizeof(double), cudaMemcpyDeviceToHost));
+    return 0;
+  }
+  // residuals and Jacobian factors at the current state, and its cost
+  int linearize(double* cost) {
+    k_linearize<<<grid_blocks(g.N, 256), 256>>>(g, 0, o->loss_function_scale);
+    return dsum(SOLVER_SUM, g.cost, nullptr, nullptr, 1, g.N, cost);
+  }
+  // column norms and gradient of the unscaled Jacobian, and the max norm of the projected gradient
+  int stats(double* gnorm) {
+    GP_CHECK(cudaMemset(g.gmax, 0, sizeof(unsigned long long)));
+    if (g.n) k_cam_stats<<<grid_blocks(g.n, 128), 128>>>(g);
+    if (g.nvp) k_point_stats<<<grid_blocks(g.nvp, 128), 128>>>(g);
+    k_scale_stats<<<grid_blocks(g.N, 256), 256>>>(g);
+    unsigned long long m = 0;
+    GP_CHECK(cudaMemcpy(&m, g.gmax, sizeof m, cudaMemcpyDeviceToHost));
+    memcpy(gnorm, &m, sizeof m);
+    return 0;
+  }
+  // norm of the variable parameters
+  int xnorm(double* r) {
+    double c, X, q, sc;
+    SOLVER_TRY(dsum(SOLVER_SUM_SQ, g.c, nullptr, fmask, 3, 3LL * g.F, &c));
+    SOLVER_TRY(dsum(SOLVER_SUM_SQ, g.X, nullptr, pvar, 3, 3 * g.P, &X));
+    SOLVER_TRY(dsum(SOLVER_SUM_SQ, g.q, nullptr, qmask, 3, 3LL * g.S, &q));
+    SOLVER_TRY(dsum(SOLVER_SUM_SQ, g.s, nullptr, smask, 1, g.N, &sc));
+    *r = sqrt(c + X + q + sc);
+    return 0;
+  }
+  // One inner step at this radius: eliminate the scales and points, build, factor and solve the reduced system,
+  // back-substitute, and the model cost change (0 unless *ok: no failed elimination or pivot).
+  int step(double radius, bool* ok, double* model) {
+    const double dmin = o->min_lm_diagonal, dmax = o->max_lm_diagonal;
+    const int n = g.n, Npad = g.Npad;
+    int zero = 0;
+    GP_CHECK(cudaMemcpy(g.bad, &zero, sizeof(int), cudaMemcpyHostToDevice));
+    k_obs_elim<<<grid_blocks(g.N, 256), 256>>>(g, radius, dmin, dmax);
+    if (g.nvp) k_point<<<grid_blocks(g.nvp, 128), 128>>>(g, radius, dmin, dmax);
+    BaDenseFlag fl{0, 0, 0.0};
+    GP_CHECK(cudaMemcpy(g.flag, &fl, sizeof fl, cudaMemcpyHostToDevice));
+    if (n) {
+      GP_CHECK(cudaMemset(g.A, 0, sizeof(double) * (size_t)Npad * Npad));
+      GP_CHECK(cudaMemset(g.rhs, 0, sizeof(double) * Npad));
+      k_rows<<<grid_blocks(n, 64), 64>>>(g, radius, dmin, dmax, pvar);
+      GP_CHECK(ba_dense_pad_identity(g.A, Npad, n, 0));
+      GP_CHECK(cudaMemcpy(g.dC, g.rhs, sizeof(double) * Npad, cudaMemcpyDeviceToDevice));
+      GP_CHECK(ba_dense_potrf(g.A, Npad, n, n, 0.0, g.dinv, g.flag, 0));
+      // b in dC, the solution back into dC; rhs is the scratch
+      GP_CHECK(ba_dense_potrs(g.A, Npad, g.dinv, 1, g.dC, g.rhs, g.flag, 0));
     }
-    vp_start.swap(ranges);
+    if (g.nvp) k_back_points<<<grid_blocks(g.nvp, 128), 128>>>(g);
+    k_back_obs<<<grid_blocks(g.N, 256), 256>>>(g, pvar);
+    GP_CHECK(cudaGetLastError());
+    int bad = 0;
+    GP_CHECK(cudaMemcpy(&bad, g.bad, sizeof(int), cudaMemcpyDeviceToHost));
+    GP_CHECK(cudaMemcpy(&fl, g.flag, sizeof fl, cudaMemcpyDeviceToHost));
+    *ok = !bad && !fl.bad;
+    *model = 0;
+    return *ok ? dsum(SOLVER_SUM, g.model, nullptr, nullptr, 1, g.N, model) : 0;
   }
-  std::vector<int64_t> obs_vp(N, -1);
-  for (int64_t k = 0; k < nvp; ++k) for (int64_t j = vp_start[2 * k]; j < vp_start[2 * k + 1]; ++j) obs_vp[j] = k;
-  for (int b = 0; b < nb; ++b) bl_count[b + 1] += bl_count[b];
-  std::vector<int64_t> bl_ent(std::max<int64_t>(1, bl_count[nb])), fill(bl_count.begin(), bl_count.end() - 1);
-  for (int64_t j = 0; j < N; ++j) for (int k = 0; k < 2; ++k) { const int b = h_blk[2 * j + k]; if (b >= 0) bl_ent[fill[b]++] = 2 * j + k; }
-
-  out->num_residuals = (int)(3 * N); out->reduced_dim = n; out->num_successful_steps = out->num_unsuccessful_steps = 0;
-  out->num_iterations = 0; out->termination_type = B200GP_FAILURE; out->solve_ms = 0; out->initial_cost = out->final_cost = 0;
-  if (N == 0) { out->termination_type = B200GP_CONVERGENCE; if (out->cost_history) out->cost_history[0] = 0.0; return 0; }
-
-  int rc = 0;
-  if (o->gpu_index >= 0) {
-    int ndev = 0; cudaGetDeviceCount(&ndev);
-    if (o->gpu_index >= ndev) return gp_fail(B200GP_ERR_INPUT, "gpu_index out of range");
-    cudaSetDevice(o->gpu_index);
+  // The candidate state from the step, its cost and the step norm.
+  int candidate(double* new_cost, double* step_norm) {
+    k_update_blocks<<<grid_blocks(std::max<int64_t>(g.n, 3 * g.P), 256), 256>>>(g, pvar);
+    k_linearize<<<grid_blocks(g.N, 256), 256>>>(g, 1, o->loss_function_scale);
+    SOLVER_TRY(dsum(SOLVER_SUM, g.cost, nullptr, nullptr, 1, g.N, new_cost));
+    double c, X, q, sc;
+    SOLVER_TRY(dsum(SOLVER_SUM_SQDIFF, g.c2, g.c, fmask, 3, 3LL * g.F, &c));
+    SOLVER_TRY(dsum(SOLVER_SUM_SQDIFF, g.X2, g.X, pvar, 3, 3 * g.P, &X));
+    SOLVER_TRY(dsum(SOLVER_SUM_SQDIFF, g.q2, g.q, qmask, 3, 3LL * g.S, &q));
+    SOLVER_TRY(dsum(SOLVER_SUM_SQDIFF, g.s2, g.s, smask, 1, g.N, &sc));
+    *step_norm = sqrt(c + X + q + sc);
+    return 0;
   }
-  GpDev g; memset(&g, 0, sizeof g);
-  g.N = N; g.P = P; g.F = F; g.S = S; g.nb = nb; g.n = n; g.Npad = Npad; g.nvp = nvp;
-  std::vector<void*> allocs;
-  uint8_t* d_pvar = nullptr; uint8_t* d_fmask = nullptr; uint8_t* d_qmask = nullptr; uint8_t* d_smask = nullptr;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  double cost = 0;
-  std::vector<uint8_t> fmask(F, 0);
-  for (int f = 0; f < F; ++f) fmask[f] = fblk[f] >= 0;
-  auto dalloc = [&](size_t bytes) -> void* { void* q = nullptr; if (cudaMalloc(&q, std::max<size_t>(bytes, 8)) != cudaSuccess) return nullptr; allocs.push_back(q); return q; };
-  auto dput = [&](const void* h, size_t bytes) -> void* { void* q = dalloc(bytes); if (q && bytes) cudaMemcpy(q, h, bytes, cudaMemcpyHostToDevice); return q; };
-#define GP_ALLOC(ptr, type, count) do { ptr = (type*)dalloc(sizeof(type) * (size_t)(count)); if (!ptr) { rc = gp_fail(B200GP_ERR_CUDA, "cudaMalloc failed"); goto cleanup; } } while (0)
-#define GP_PUT(ptr, type, vec) do { ptr = (type*)dput((vec).data(), sizeof(type) * (vec).size()); if (!ptr) { rc = gp_fail(B200GP_ERR_CUDA, "cudaMalloc failed"); goto cleanup; } } while (0)
-  {
-    std::vector<double> hc(p->frame_centers, p->frame_centers + 3LL * F), hX(p->points, p->points + 3 * P), hq(p->cams_in_rig ? p->cams_in_rig : nullptr, p->cams_in_rig ? p->cams_in_rig + 3LL * S : nullptr);
-    std::vector<int64_t> vps(vp_start.begin(), vp_start.end());
-    GP_PUT(g.ray, const double, h_ray); GP_PUT(g.off, const double, h_off); GP_PUT(g.R, const double, h_R); GP_PUT(g.w, const double, h_w);
-    GP_PUT(g.fr, const int, h_fr); GP_PUT(g.sen, const int, h_sen); GP_PUT(g.blk, const int, h_blk); GP_PUT(g.pt, const int64_t, h_pt);
-    GP_PUT(g.svar, const uint8_t, h_svar); GP_PUT(g.vp_start, const int64_t, vps); GP_PUT(g.vp_pt, const int64_t, vp_pt);
-    GP_PUT(g.obs_vp, const int64_t, obs_vp);
-    GP_PUT(g.bl_start, const int64_t, bl_count); GP_PUT(g.bl_ent, const int64_t, bl_ent);
-    GP_PUT(g.blk_frame, const int, blk_frame); GP_PUT(g.blk_sensor, const int, blk_sensor);
-    GP_PUT(g.c, double, hc); GP_PUT(g.X, double, hX); GP_PUT(g.q, double, hq); GP_PUT(g.s, double, h_s);
-    GP_PUT(g.c2, double, hc); GP_PUT(g.X2, double, hX); GP_PUT(g.q2, double, hq); GP_PUT(g.s2, double, h_s);
-    GP_PUT(d_pvar, uint8_t, pvar); GP_PUT(d_fmask, uint8_t, fmask); GP_PUT(d_qmask, uint8_t, sensor_used); GP_PUT(d_smask, uint8_t, h_svar);
+  // the candidate becomes the current state, and the next candidate starts from it
+  int accept() {
+    std::swap(g.c, g.c2); std::swap(g.X, g.X2); std::swap(g.q, g.q2); std::swap(g.s, g.s2);
+    GP_CHECK(cudaMemcpy(g.c2, g.c, sizeof(double) * 3 * g.F, cudaMemcpyDeviceToDevice));
+    GP_CHECK(cudaMemcpy(g.X2, g.X, sizeof(double) * 3 * g.P, cudaMemcpyDeviceToDevice));
+    if (g.S) GP_CHECK(cudaMemcpy(g.q2, g.q, sizeof(double) * 3 * g.S, cudaMemcpyDeviceToDevice));
+    return 0;
   }
-  GP_ALLOC(g.r, double, 3 * N); GP_ALLOC(g.u, double, N); GP_ALLOC(g.js, double, 3 * N); GP_ALLOC(g.cost, double, N);
-  GP_ALLOC(g.Dc, double, n); GP_ALLOC(g.Dp, double, 3 * P); GP_ALLOC(g.Ds, double, N);
-  GP_ALLOC(g.nc, double, n); GP_ALLOC(g.np, double, 3 * P); GP_ALLOC(g.ns, double, N);
-  GP_ALLOC(g.gc, double, n); GP_ALLOC(g.gp, double, 3 * P); GP_ALLOC(g.gs, double, N);
-  GP_ALLOC(g.P9, double, 9 * N); GP_ALLOC(g.e, double, 3 * N); GP_ALLOC(g.Hss, double, N); GP_ALLOC(g.gss, double, N);
-  GP_ALLOC(g.E, double, 18 * N); GP_ALLOC(g.Fm, double, 18 * N);
-  GP_ALLOC(g.Hinv, double, 9 * P); GP_ALLOC(g.h, double, 3 * P); GP_ALLOC(g.gpt, double, 3 * P);
-  GP_ALLOC(g.A, double, (size_t)Npad * Npad); GP_ALLOC(g.rhs, double, Npad); GP_ALLOC(g.dC, double, Npad);
-  GP_ALLOC(g.dX, double, 3 * P); GP_ALLOC(g.ds, double, N); GP_ALLOC(g.model, double, N);
-  GP_ALLOC(g.dinv, double, (size_t)Npad * BA_TILE); GP_ALLOC(g.flag, BaDenseFlag, 1); GP_ALLOC(g.bad, int, 1);
-  GP_ALLOC(g.gmax, unsigned long long, 1); GP_ALLOC(g.red, double, GP_RG + 8);
-  GP_CUDA(cudaMemset(g.dX, 0, sizeof(double) * 3 * std::max<int64_t>(P, 1)));
-  GP_CUDA(cudaMemset(g.ns, 0, sizeof(double) * N));
-  GP_CUDA(cudaMemset(g.np, 0, sizeof(double) * 3 * std::max<int64_t>(P, 1)));
-  GP_CUDA(cudaEventCreate(&ev0)); GP_CUDA(cudaEventCreate(&ev1));
-  GP_CUDA(cudaEventRecord(ev0));
-  {
-    const double a = o->loss_function_scale, dmin = o->min_lm_diagonal, dmax = o->max_lm_diagonal;
-    auto dsum = [&](const double* x, const double* y, const uint8_t* mask, int stride, int64_t cnt, int mode) -> double {
-      double r = 0;
-      if (cnt <= 0) return 0.0;
-      k_reduce1<<<GP_RG, GP_RB>>>(x, y, mask, stride, cnt, mode, g.red);
-      k_reduce2<<<1, GP_RB>>>(g.red, g.red + GP_RG);
-      cudaMemcpy(&r, g.red + GP_RG, sizeof(double), cudaMemcpyDeviceToHost);
-      return r;
-    };
-    auto linearize = [&]() -> double { k_linearize<<<gp_blocks(N, 256), 256>>>(g, 0, a); return dsum(g.cost, nullptr, nullptr, 1, N, 0); };
-    auto stats = [&]() -> double {
-      cudaMemset(g.gmax, 0, sizeof(unsigned long long));
-      if (n) k_cam_stats<<<gp_blocks(n, 128), 128>>>(g);
-      if (nvp) k_point_stats<<<gp_blocks(nvp, 128), 128>>>(g);
-      k_scale_stats<<<gp_blocks(N, 256), 256>>>(g);
-      unsigned long long m = 0; cudaMemcpy(&m, g.gmax, sizeof m, cudaMemcpyDeviceToHost);
-      double v; memcpy(&v, &m, sizeof v); return v;
-    };
-    cost = linearize();
-    out->initial_cost = cost;
-    if (out->cost_history) out->cost_history[0] = cost;
+  // The LM iterations from the uploaded state.  Sets the termination type, the step counts and the cost history, and
+  // leaves the last accepted state in (c, X, q, s) and its cost in *cost.
+  int minimize(double* cost) {
+    SOLVER_TRY(linearize(cost));
+    out->initial_cost = *cost;
+    if (out->cost_history) out->cost_history[0] = *cost;
     double radius = o->initial_trust_region_radius, decrease_factor = 2.0;
     int iter = 0;
     out->termination_type = B200GP_NO_CONVERGENCE;
-    double gnorm = stats();
-    if (n) k_jacobi<<<gp_blocks(n, 256), 256>>>(g.Dc, g.nc, n);
-    if (P) k_jacobi<<<gp_blocks(3 * P, 256), 256>>>(g.Dp, g.np, 3 * P);
-    k_jacobi<<<gp_blocks(N, 256), 256>>>(g.Ds, g.ns, N);
-    // x norm over the variable parameters (constant in the inner loop)
-    auto xnorm = [&]() {
-      return sqrt(dsum(g.c, nullptr, d_fmask, 3, 3LL * F, 2) + dsum(g.X, nullptr, d_pvar, 3, 3 * P, 2) +
-                  dsum(g.q, nullptr, d_qmask, 3, 3LL * S, 2) + dsum(g.s, nullptr, d_smask, 1, N, 2));
-    };
+    double gnorm;
+    SOLVER_TRY(stats(&gnorm));
+    if (g.n) k_jacobi<<<grid_blocks(g.n, 256), 256>>>(g.Dc, g.nc, g.n);
+    if (g.P) k_jacobi<<<grid_blocks(3 * g.P, 256), 256>>>(g.Dp, g.np, 3 * g.P);
+    k_jacobi<<<grid_blocks(g.N, 256), 256>>>(g.Ds, g.ns, g.N);
     for (;;) {
-      if (gnorm <= o->gradient_tolerance) { out->termination_type = B200GP_CONVERGENCE; break; }
-      const double x_norm = xnorm();
+      if (gnorm <= o->gradient_tolerance) { out->termination_type = B200GP_CONVERGENCE; return 0; }
+      double x_norm;   // constant in the inner loop
+      SOLVER_TRY(xnorm(&x_norm));
       bool accepted = false;
       while (!accepted) {
-        if (iter >= o->max_num_iterations) goto done;
+        if (iter >= o->max_num_iterations) return 0;
         ++iter;
-        int zero = 0;
-        GP_CUDA(cudaMemcpy(g.bad, &zero, sizeof(int), cudaMemcpyHostToDevice));
-        k_obs_elim<<<gp_blocks(N, 256), 256>>>(g, radius, dmin, dmax);
-        if (nvp) k_point<<<gp_blocks(nvp, 128), 128>>>(g, radius, dmin, dmax);
-        BaDenseFlag fl{0, 0, 0.0};
-        GP_CUDA(cudaMemcpy(g.flag, &fl, sizeof fl, cudaMemcpyHostToDevice));
-        if (n) {
-          GP_CUDA(cudaMemset(g.A, 0, sizeof(double) * (size_t)Npad * Npad));
-          GP_CUDA(cudaMemset(g.rhs, 0, sizeof(double) * Npad));
-          k_rows<<<gp_blocks(n, 64), 64>>>(g, radius, dmin, dmax, d_pvar);
-          if (Npad > n) k_pad_identity<<<gp_blocks(Npad - n, 64), 64>>>(g.A, n, Npad);
-          GP_CUDA(cudaMemcpy(g.dC, g.rhs, sizeof(double) * Npad, cudaMemcpyDeviceToDevice));
-          GP_CUDA(ba_dense_potrf(g.A, Npad, n, n, 0.0, g.dinv, g.flag, 0));
-          // b in dC, the solution back into dC; rhs is the scratch
-          GP_CUDA(ba_dense_potrs(g.A, Npad, g.dinv, 1, g.dC, g.rhs, g.flag, 0));
-        }
-        if (nvp) k_back_points<<<gp_blocks(nvp, 128), 128>>>(g);
-        k_back_obs<<<gp_blocks(N, 256), 256>>>(g, d_pvar);
-        GP_CUDA(cudaGetLastError());
-        int bad = 0; GP_CUDA(cudaMemcpy(&bad, g.bad, sizeof(int), cudaMemcpyDeviceToHost));
-        GP_CUDA(cudaMemcpy(&fl, g.flag, sizeof fl, cudaMemcpyDeviceToHost));
-        const bool ok = !bad && !fl.bad;
-        double model = 0, new_cost = cost, rho = 0;
-        if (ok) model = dsum(g.model, nullptr, nullptr, 1, N, 0);
+        bool ok; double model;
+        SOLVER_TRY(step(radius, &ok, &model));
+        double new_cost = *cost, rho = 0;
         if (ok && model > 0) {
-                    k_update_blocks<<<gp_blocks(std::max<int64_t>(n, 3 * P), 256), 256>>>(g, d_pvar);
-          k_linearize<<<gp_blocks(N, 256), 256>>>(g, 1, a);
-          new_cost = dsum(g.cost, nullptr, nullptr, 1, N, 0);
-          rho = (cost - new_cost) / model;
-          // ParameterToleranceReached, then FunctionToleranceReached (checked on every step, as Ceres does)
-          const double step = sqrt(dsum(g.c2, g.c, d_fmask, 3, 3LL * F, 1) + dsum(g.X2, g.X, d_pvar, 3, 3 * P, 1) +
-                                   dsum(g.q2, g.q, d_qmask, 3, 3LL * S, 1) + dsum(g.s2, g.s, d_smask, 1, N, 1));
-          // a converged candidate is not taken: Ceres returns with the last accepted parameters
-          if (step / (x_norm + o->parameter_tolerance) <= o->parameter_tolerance ||
-              fabs(cost - new_cost) <= o->function_tolerance * cost) {
+          double step_norm;
+          SOLVER_TRY(candidate(&new_cost, &step_norm));
+          rho = (*cost - new_cost) / model;
+          // ParameterToleranceReached, then FunctionToleranceReached (checked on every step, as Ceres does); a converged
+          // candidate is not taken: Ceres returns with the last accepted parameters
+          if (step_norm / (x_norm + o->parameter_tolerance) <= o->parameter_tolerance ||
+              fabs(*cost - new_cost) <= o->function_tolerance * *cost) {
             out->termination_type = B200GP_CONVERGENCE;
-            if (out->cost_history) out->cost_history[iter] = cost;
+            if (out->cost_history) out->cost_history[iter] = *cost;
             out->num_iterations = iter;
-            goto done;
+            return 0;
           }
         }
         if (ok && model > 0 && rho > o->min_relative_decrease) {
           accepted = true;
           out->num_successful_steps++;
-          std::swap(g.c, g.c2); std::swap(g.X, g.X2); std::swap(g.q, g.q2); std::swap(g.s, g.s2);
-          GP_CUDA(cudaMemcpy(g.c2, g.c, sizeof(double) * 3 * F, cudaMemcpyDeviceToDevice));
-          GP_CUDA(cudaMemcpy(g.X2, g.X, sizeof(double) * 3 * P, cudaMemcpyDeviceToDevice));
-          if (S) GP_CUDA(cudaMemcpy(g.q2, g.q, sizeof(double) * 3 * S, cudaMemcpyDeviceToDevice));
-          cost = linearize();
-          gnorm = stats();
+          SOLVER_TRY(accept());
+          SOLVER_TRY(linearize(cost));
+          SOLVER_TRY(stats(&gnorm));
           const double t = 2.0 * rho - 1.0;
           radius = std::min(o->max_trust_region_radius, radius / std::max(1.0 / 3.0, 1.0 - t * t * t));
           decrease_factor = 2.0;
@@ -745,30 +727,95 @@ extern "C" int b200gp_solve(const b200gp_options* o, b200gp_problem* p, b200gp_s
           radius /= decrease_factor;
           decrease_factor *= 2.0;
         }
-        if (out->cost_history) out->cost_history[iter] = cost;
+        if (out->cost_history) out->cost_history[iter] = *cost;
         out->num_iterations = iter;
-        if (!accepted && radius < o->min_trust_region_radius) { out->termination_type = B200GP_CONVERGENCE; goto done; }
+        if (!accepted && radius < o->min_trust_region_radius) { out->termination_type = B200GP_CONVERGENCE; return 0; }
       }
     }
-  done:
-    GP_CUDA(cudaEventRecord(ev1));
-    GP_CUDA(cudaEventSynchronize(ev1));
-    float ms = 0; cudaEventElapsedTime(&ms, ev0, ev1);
-    out->solve_ms = ms; out->final_cost = cost;
-    // write back the variable blocks (constants stay bit-identical)
-    std::vector<double> hc(3LL * F), hX(3 * P), hq(3LL * S), hs(N);
-    GP_CUDA(cudaMemcpy(hc.data(), g.c, sizeof(double) * 3 * F, cudaMemcpyDeviceToHost));
-    GP_CUDA(cudaMemcpy(hX.data(), g.X, sizeof(double) * 3 * P, cudaMemcpyDeviceToHost));
-    if (S) GP_CUDA(cudaMemcpy(hq.data(), g.q, sizeof(double) * 3 * S, cudaMemcpyDeviceToHost));
-    GP_CUDA(cudaMemcpy(hs.data(), g.s, sizeof(double) * N, cudaMemcpyDeviceToHost));
-    for (int f = 0; f < F; ++f) if (fblk[f] >= 0) for (int m = 0; m < 3; ++m) p->frame_centers[3 * f + m] = hc[3 * f + m];
-    for (int64_t q = 0; q < P; ++q) if (pvar[q]) for (int m = 0; m < 3; ++m) p->points[3 * q + m] = hX[3 * q + m];
-    for (int s = 0; s < S; ++s) if (sblk[s] >= 0) for (int m = 0; m < 3; ++m) p->cams_in_rig[3 * s + m] = hq[3 * s + m];
-    for (int64_t j = 0; j < N; ++j) if (h_svar[j]) p->obs_scale[perm[j]] = hs[j];
   }
-cleanup:
-  for (void* q : allocs) cudaFree(q);
-  if (ev0) cudaEventDestroy(ev0);
-  if (ev1) cudaEventDestroy(ev1);
-  return rc;
+};
+
+// GpDev's buffers: the layout and the initial state uploaded (current and candidate), the work arrays allocated
+static int gp_upload(const b200gp_problem* p, const GpLayout& L, SolverBuffers& pool, GpSolve& s) {
+  const int F = p->num_frames, S = p->num_sensors; const int64_t P = p->num_points, N = p->num_observations;
+  const int n = L.n, Npad = L.Npad;
+  GpDev& g = s.g;
+  memset(&g, 0, sizeof g);
+  g.N = N; g.P = P; g.F = F; g.S = S; g.nb = L.nb; g.n = n; g.Npad = Npad; g.nvp = L.nvp;
+  const std::vector<double> hc(p->frame_centers, p->frame_centers + 3LL * F), hX(p->points, p->points + 3 * P),
+      hq(p->cams_in_rig ? p->cams_in_rig : nullptr, p->cams_in_rig ? p->cams_in_rig + 3LL * S : nullptr);
+  GP_CHECK(pool.upload(&g.ray, L.ray)); GP_CHECK(pool.upload(&g.off, L.off)); GP_CHECK(pool.upload(&g.R, L.R));
+  GP_CHECK(pool.upload(&g.w, L.w)); GP_CHECK(pool.upload(&g.fr, L.fr)); GP_CHECK(pool.upload(&g.sen, L.sen));
+  GP_CHECK(pool.upload(&g.blk, L.blk)); GP_CHECK(pool.upload(&g.pt, L.pt)); GP_CHECK(pool.upload(&g.svar, L.svar));
+  GP_CHECK(pool.upload(&g.vp_start, L.vp_start)); GP_CHECK(pool.upload(&g.vp_pt, L.vp_pt));
+  GP_CHECK(pool.upload(&g.obs_vp, L.obs_vp));
+  GP_CHECK(pool.upload(&g.bl_start, L.bl_start)); GP_CHECK(pool.upload(&g.bl_ent, L.bl_ent));
+  GP_CHECK(pool.upload(&g.blk_frame, L.blk_frame)); GP_CHECK(pool.upload(&g.blk_sensor, L.blk_sensor));
+  GP_CHECK(pool.upload(&g.c, hc)); GP_CHECK(pool.upload(&g.X, hX)); GP_CHECK(pool.upload(&g.q, hq)); GP_CHECK(pool.upload(&g.s, L.s));
+  GP_CHECK(pool.upload(&g.c2, hc)); GP_CHECK(pool.upload(&g.X2, hX)); GP_CHECK(pool.upload(&g.q2, hq)); GP_CHECK(pool.upload(&g.s2, L.s));
+  GP_CHECK(pool.upload(&s.pvar, L.pvar)); GP_CHECK(pool.upload(&s.fmask, L.fmask)); GP_CHECK(pool.upload(&s.qmask, L.sensor_used));
+  GP_CHECK(pool.upload(&s.smask, L.svar));
+  GP_CHECK(pool.alloc(&g.r, 3 * N)); GP_CHECK(pool.alloc(&g.u, N)); GP_CHECK(pool.alloc(&g.js, 3 * N)); GP_CHECK(pool.alloc(&g.cost, N));
+  GP_CHECK(pool.alloc(&g.Dc, n)); GP_CHECK(pool.alloc(&g.Dp, 3 * P)); GP_CHECK(pool.alloc(&g.Ds, N));
+  GP_CHECK(pool.alloc(&g.nc, n)); GP_CHECK(pool.alloc(&g.np, 3 * P)); GP_CHECK(pool.alloc(&g.ns, N));
+  GP_CHECK(pool.alloc(&g.gc, n)); GP_CHECK(pool.alloc(&g.gp, 3 * P)); GP_CHECK(pool.alloc(&g.gs, N));
+  GP_CHECK(pool.alloc(&g.P9, 9 * N)); GP_CHECK(pool.alloc(&g.e, 3 * N)); GP_CHECK(pool.alloc(&g.Hss, N)); GP_CHECK(pool.alloc(&g.gss, N));
+  GP_CHECK(pool.alloc(&g.E, 18 * N)); GP_CHECK(pool.alloc(&g.Fm, 18 * N));
+  GP_CHECK(pool.alloc(&g.Hinv, 9 * P)); GP_CHECK(pool.alloc(&g.h, 3 * P)); GP_CHECK(pool.alloc(&g.gpt, 3 * P));
+  GP_CHECK(pool.alloc(&g.A, (size_t)Npad * Npad)); GP_CHECK(pool.alloc(&g.rhs, Npad)); GP_CHECK(pool.alloc(&g.dC, Npad));
+  GP_CHECK(pool.alloc(&g.dX, 3 * P)); GP_CHECK(pool.alloc(&g.ds, N)); GP_CHECK(pool.alloc(&g.model, N));
+  GP_CHECK(pool.alloc(&g.dinv, (size_t)Npad * BA_TILE)); GP_CHECK(pool.alloc(&g.flag, 1)); GP_CHECK(pool.alloc(&g.bad, 1));
+  GP_CHECK(pool.alloc(&g.gmax, 1)); GP_CHECK(pool.alloc(&g.red, GP_RG + 8));
+  GP_CHECK(cudaMemset(g.dX, 0, sizeof(double) * 3 * std::max<int64_t>(P, 1)));
+  GP_CHECK(cudaMemset(g.ns, 0, sizeof(double) * N));
+  GP_CHECK(cudaMemset(g.np, 0, sizeof(double) * 3 * std::max<int64_t>(P, 1)));
+  return 0;
+}
+
+// the variable blocks back into the caller's arrays (constants stay bit-identical)
+static int gp_write_back(const GpLayout& L, const GpDev& g, b200gp_problem* p) {
+  const int F = g.F, S = g.S; const int64_t P = g.P, N = g.N;
+  std::vector<double> hc(3LL * F), hX(3 * P), hq(3LL * S), hs(N);
+  GP_CHECK(cudaMemcpy(hc.data(), g.c, sizeof(double) * 3 * F, cudaMemcpyDeviceToHost));
+  GP_CHECK(cudaMemcpy(hX.data(), g.X, sizeof(double) * 3 * P, cudaMemcpyDeviceToHost));
+  if (S) GP_CHECK(cudaMemcpy(hq.data(), g.q, sizeof(double) * 3 * S, cudaMemcpyDeviceToHost));
+  GP_CHECK(cudaMemcpy(hs.data(), g.s, sizeof(double) * N, cudaMemcpyDeviceToHost));
+  for (int f = 0; f < F; ++f) if (L.fblk[f] >= 0) for (int m = 0; m < 3; ++m) p->frame_centers[3 * f + m] = hc[3 * f + m];
+  for (int64_t q = 0; q < P; ++q) if (L.pvar[q]) for (int m = 0; m < 3; ++m) p->points[3 * q + m] = hX[3 * q + m];
+  for (int s = 0; s < S; ++s) if (L.sblk[s] >= 0) for (int m = 0; m < 3; ++m) p->cams_in_rig[3 * s + m] = hq[3 * s + m];
+  for (int64_t j = 0; j < N; ++j) if (L.svar[j]) p->obs_scale[L.perm[j]] = hs[j];
+  return 0;
+}
+
+extern "C" int b200gp_solve(const b200gp_options* o, b200gp_problem* p, b200gp_summary* out) {
+  g_gp_err.clear();
+  if (!o || !p || !out) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "null argument");
+  SOLVER_TRY(gp_check(o, p));
+  GpLayout L;
+  SOLVER_TRY(gp_layout(o, p, L));
+  const int64_t N = p->num_observations;
+  out->num_residuals = (int)(3 * N); out->reduced_dim = L.n; out->num_successful_steps = out->num_unsuccessful_steps = 0;
+  out->num_iterations = 0; out->termination_type = B200GP_FAILURE; out->solve_ms = 0; out->initial_cost = out->final_cost = 0;
+  if (N == 0) { out->termination_type = B200GP_CONVERGENCE; if (out->cost_history) out->cost_history[0] = 0.0; return 0; }
+
+  if (o->gpu_index >= 0) {
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess) ndev = 0;   // no usable device: the index is out of range
+    if (o->gpu_index >= ndev) return solver_fail(g_gp_err, B200GP_ERR_INPUT, "gpu_index out of range");
+    GP_CHECK(cudaSetDevice(o->gpu_index));
+  }
+  SolverBuffers pool;
+  GpSolve s{o, out};
+  SOLVER_TRY(gp_upload(p, L, pool, s));
+  cudaEvent_t ev0, ev1;
+  GP_CHECK(pool.event(&ev0)); GP_CHECK(pool.event(&ev1));
+  GP_CHECK(cudaEventRecord(ev0));
+  double cost = 0;
+  SOLVER_TRY(s.minimize(&cost));
+  GP_CHECK(cudaEventRecord(ev1));
+  GP_CHECK(cudaEventSynchronize(ev1));
+  float ms = 0;
+  GP_CHECK(cudaEventElapsedTime(&ms, ev0, ev1));
+  out->solve_ms = ms; out->final_cost = cost;
+  return gp_write_back(L, s.g, p);
 }

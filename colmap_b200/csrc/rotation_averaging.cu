@@ -15,8 +15,6 @@
 // Cholesky factorisation fails, which is reported here as B200RA_FACTORIZATION_FAILED (DESIGN.md, "Rotation averaging").
 #include <cuda_runtime.h>
 #include <math.h>
-#include <stdarg.h>
-#include <stdio.h>
 #include <string.h>
 
 #include <algorithm>
@@ -25,14 +23,10 @@
 
 #include "../../include/b200_rotation_averaging.h"
 #include "ba_dense_f64.h"
+#include "solver_host.cuh"
 
 static thread_local std::string g_ra_err;
-static int ra_fail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof buf, fmt, ap); va_end(ap);
-  g_ra_err = buf;
-  return code;
-}
+#define RA_CHECK(call) SOLVER_CUDA(g_ra_err, B200RA_ERR_CUDA, call)
 extern "C" const char* b200ra_last_error(void) { return g_ra_err.c_str(); }
 
 extern "C" void b200ra_options_init(b200ra_options* o) {
@@ -196,11 +190,6 @@ __global__ void k_ra_build(RaDev g, int axis_y, const double* w, double ridge, d
   }
   if (b == g.gauge && (axis_y || g.gdof == 3)) col[c] += 1.0;
   if (ridge > 0.0) col[c] += ridge;
-}
-
-__global__ void k_ra_pad_identity(double* M, int n, int Npad) {
-  const int i = n + blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < Npad) M[(long long)i * Npad + i] = 1.0;
 }
 
 // out = A^T diag(w) v in parameter order, one thread per block: the incident rows in list order, then the gauge (weight 1)
@@ -371,335 +360,367 @@ __global__ void __launch_bounds__(RA_CB) k_ra_update_cameras(RaDev g) {
   ra_log(R, g.rot + g.off[b]);
 }
 
-// deterministic sums: fixed grid, fixed per-thread order, fixed tree.  mode 0: sum a; 1: sum a^2
-#define RA_RB 256
-#define RA_RG 256
-__global__ void k_ra_reduce1(const double* a, int64_t n, int mode, double* part) {
-  __shared__ double sh[RA_RB];
-  double s = 0;
-  for (int64_t i = blockIdx.x * (int64_t)RA_RB + threadIdx.x; i < n; i += (int64_t)RA_RG * RA_RB) s += mode ? a[i] * a[i] : a[i];
-  sh[threadIdx.x] = s;
-  __syncthreads();
-  for (int o = RA_RB / 2; o; o >>= 1) { if (threadIdx.x < o) sh[threadIdx.x] += sh[threadIdx.x + o]; __syncthreads(); }
-  if (!threadIdx.x) part[blockIdx.x] = sh[0];
-}
-__global__ void k_ra_reduce2(const double* part, double* out) {
-  __shared__ double sh[RA_RG];
-  sh[threadIdx.x] = part[threadIdx.x];
-  __syncthreads();
-  for (int o = RA_RG / 2; o; o >>= 1) { if (threadIdx.x < o) sh[threadIdx.x] += sh[threadIdx.x + o]; __syncthreads(); }
-  if (!threadIdx.x) *out = sh[0];
-}
 
 // ------------------------------------------------------------------------------------------------ host
-static inline unsigned ra_blocks(int64_t n, int t) { return (unsigned)std::max<int64_t>(1, (n + t - 1) / t); }
-static bool ra_finite(const double* a, int64_t n) { for (int64_t i = 0; i < n; ++i) if (!std::isfinite(a[i])) return false; return true; }
+#define RA_RG 256   // CTAs of the deterministic sums
 
-#define RA_CUDA(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { rc = ra_fail(B200RA_ERR_CUDA, "%s: %s", #x, cudaGetErrorString(e_)); goto cleanup; } } while (0)
+// The parameter, residual and axis layout of a problem and its block -> incident-pair lists (RaDev); the checks run
+// interleaved with the layout because their messages use it.  Arrays copied to the device hold at least one element.
+struct RaLayout {
+  int F, C, P, nb, np, n_xz, n_y, gauge, gdof, same_y, Np_xz, Np_y;
+  int64_t m;
+  std::vector<int> off, dof, cx, xz_blk, roff, cstart, cfr;
+  std::vector<int> bstart, bent, f1, f2, c1, c2;
+  std::vector<uint8_t> pdof;
+  std::vector<double> rw, rwrow, rw2, R, ang, xz;
+};
 
-extern "C" int b200ra_solve(const b200ra_options* o, b200ra_problem* p, b200ra_summary* out) {
-  g_ra_err.clear();
-  if (!o || !p || !out) return ra_fail(B200RA_ERR_INPUT, "null argument");
+static int ra_layout(const b200ra_options* o, const b200ra_problem* p, RaLayout& L) {
   // ---- options
   if (o->max_num_l1_iterations < 0 || o->max_num_irls_iterations < 0 || !(o->l1_step_convergence_threshold >= 0) ||
       !(o->irls_step_convergence_threshold >= 0) || !(o->irls_loss_parameter_sigma > 0) ||
       !std::isfinite(o->irls_loss_parameter_sigma) || !(o->ridge_regularization >= 0) ||
       !std::isfinite(o->ridge_regularization) || (o->weight_type != B200RA_GEMAN_MCCLURE && o->weight_type != B200RA_HALF_NORM))
-    return ra_fail(B200RA_ERR_INPUT, "invalid solver options");
+    return solver_fail(g_ra_err, B200RA_ERR_INPUT, "invalid solver options");
   // ---- problem
   const int F = p->num_frames, C = p->num_cameras, P = p->num_pairs;
-  if (F < 1 || C < 0 || P < 0) return ra_fail(B200RA_ERR_INPUT, "need at least one frame and non-negative sizes");
+  if (F < 1 || C < 0 || P < 0) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "need at least one frame and non-negative sizes");
   if (!p->frame_dof || !p->rotations || (P && (!p->pair_frame1 || !p->pair_frame2 || !p->pair_dof)))
-    return ra_fail(B200RA_ERR_INPUT, "missing array");
-  if (C && (!p->cam_frame_start || !p->cam_frames)) return ra_fail(B200RA_ERR_INPUT, "estimated cameras need the camera -> frames lists");
+    return solver_fail(g_ra_err, B200RA_ERR_INPUT, "missing array");
+  if (C && (!p->cam_frame_start || !p->cam_frames)) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "estimated cameras need the camera -> frames lists");
   const int nb = F + C;
-  std::vector<int> off(nb), dof(nb), cx(nb, -1), xz_blk;
+  L.F = F; L.C = C; L.P = P; L.nb = nb;
+  L.off.resize(nb); L.dof.resize(nb); L.cx.assign(nb, -1);
   int np = 0;
   for (int b = 0; b < nb; ++b) {
     const int d = b < F ? p->frame_dof[b] : 3;
-    if (d != 1 && d != 3) return ra_fail(B200RA_ERR_INPUT, "frame %d: dof %d is neither 1 nor 3", b, d);
-    off[b] = np; dof[b] = d; np += d;
-    if (d == 3) { cx[b] = (int)xz_blk.size(); xz_blk.push_back(b); }
+    if (d != 1 && d != 3) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "frame %d: dof %d is neither 1 nor 3", b, d);
+    L.off[b] = np; L.dof[b] = d; np += d;
+    if (d == 3) { L.cx[b] = (int)L.xz_blk.size(); L.xz_blk.push_back(b); }
   }
-  if (!ra_finite(p->rotations, np)) return ra_fail(B200RA_ERR_INPUT, "non-finite rotation");
-  const int n_xz = (int)xz_blk.size(), n_y = nb;
-  std::vector<int> roff(P);
-  std::vector<double> rw(P, 1.0);
+  L.np = np;
+  if (!all_finite(p->rotations, np)) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "non-finite rotation");
+  const int n_xz = (int)L.xz_blk.size(), n_y = nb;
+  if (L.xz_blk.empty()) L.xz_blk.push_back(0);
+  L.roff.assign(std::max(P, 1), 0);
+  L.rw.assign(std::max(P, 1), 1.0);
   int64_t m = 0;
   for (int q = 0; q < P; ++q) {
     const int a = p->pair_frame1[q], b = p->pair_frame2[q];
     const int c1 = p->pair_cam1 ? p->pair_cam1[q] : -1, c2 = p->pair_cam2 ? p->pair_cam2[q] : -1;
-    if (a < 0 || a >= F || b < 0 || b >= F) return ra_fail(B200RA_ERR_INPUT, "pair %d: frame out of range", q);
-    if (c1 < -1 || c1 >= C || c2 < -1 || c2 >= C) return ra_fail(B200RA_ERR_INPUT, "pair %d: camera out of range", q);
+    if (a < 0 || a >= F || b < 0 || b >= F) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "pair %d: frame out of range", q);
+    if (c1 < -1 || c1 >= C || c2 < -1 || c2 >= C) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "pair %d: camera out of range", q);
     const int d = p->pair_dof[q];
     if (d == 1) {
-      if (dof[a] != 1 || dof[b] != 1) return ra_fail(B200RA_ERR_INPUT, "pair %d: a 1-DOF pair needs two 1-DOF frames", q);
-      if (c1 >= 0 || c2 >= 0) return ra_fail(B200RA_ERR_INPUT, "pair %d: a 1-DOF pair cannot have estimated cameras", q);
-      if (!p->pair_angle || !p->pair_xz_error) return ra_fail(B200RA_ERR_INPUT, "1-DOF pairs need pair_angle and pair_xz_error");
+      if (L.dof[a] != 1 || L.dof[b] != 1) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "pair %d: a 1-DOF pair needs two 1-DOF frames", q);
+      if (c1 >= 0 || c2 >= 0) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "pair %d: a 1-DOF pair cannot have estimated cameras", q);
+      if (!p->pair_angle || !p->pair_xz_error) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "1-DOF pairs need pair_angle and pair_xz_error");
       if (!std::isfinite(p->pair_angle[q]) || !(p->pair_xz_error[q] >= 0) || !std::isfinite(p->pair_xz_error[q]))
-        return ra_fail(B200RA_ERR_INPUT, "pair %d: non-finite angle or xz_error", q);
+        return solver_fail(g_ra_err, B200RA_ERR_INPUT, "pair %d: non-finite angle or xz_error", q);
     } else if (d == 3) {
-      if (dof[a] == 1 && dof[b] == 1) return ra_fail(B200RA_ERR_INPUT, "pair %d: a 3-DOF pair between two 1-DOF frames", q);
-      if (!p->pair_R || !ra_finite(p->pair_R + 9LL * q, 9)) return ra_fail(B200RA_ERR_INPUT, "pair %d: missing or non-finite R_cam2_from_cam1", q);
+      if (L.dof[a] == 1 && L.dof[b] == 1) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "pair %d: a 3-DOF pair between two 1-DOF frames", q);
+      if (!p->pair_R || !all_finite(p->pair_R + 9LL * q, 9)) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "pair %d: missing or non-finite R_cam2_from_cam1", q);
     } else {
-      return ra_fail(B200RA_ERR_INPUT, "pair %d: dof %d is neither 1 nor 3", q, d);
+      return solver_fail(g_ra_err, B200RA_ERR_INPUT, "pair %d: dof %d is neither 1 nor 3", q, d);
     }
     if (p->pair_reweighting) {
-      rw[q] = p->pair_reweighting[q];
-      if (!(rw[q] >= 0) || !std::isfinite(rw[q])) return ra_fail(B200RA_ERR_INPUT, "pair %d: reweighting must be finite and >= 0", q);
+      L.rw[q] = p->pair_reweighting[q];
+      if (!(L.rw[q] >= 0) || !std::isfinite(L.rw[q])) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "pair %d: reweighting must be finite and >= 0", q);
     }
-    roff[q] = (int)m; m += d;
+    L.roff[q] = (int)m; m += d;
   }
   const int gauge = p->gauge_frame;
-  if (gauge < 0 || gauge >= F) return ra_fail(B200RA_ERR_INPUT, "gauge frame %d out of range", gauge);
-  if (!ra_finite(p->gauge_rotation, 3)) return ra_fail(B200RA_ERR_INPUT, "non-finite gauge rotation");
-  const int gdof = dof[gauge];
+  if (gauge < 0 || gauge >= F) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "gauge frame %d out of range", gauge);
+  if (!all_finite(p->gauge_rotation, 3)) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "non-finite gauge rotation");
+  const int gdof = L.dof[gauge];
   m += gdof;
-  if (m > 0x7fffffff - 16) return ra_fail(B200RA_ERR_INPUT, "too many residual rows");
-  std::vector<int> cstart(C + 1, 0), cfr;
+  if (m > 0x7fffffff - 16) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "too many residual rows");
+  L.cstart.assign(C + 1, 0);
+  L.cfr.assign(1, 0);
   if (C) {
-    if (p->cam_frame_start[0] != 0) return ra_fail(B200RA_ERR_INPUT, "cam_frame_start[0] must be 0");
+    if (p->cam_frame_start[0] != 0) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "cam_frame_start[0] must be 0");
     for (int c = 0; c < C; ++c) {
-      cstart[c + 1] = p->cam_frame_start[c + 1];
-      if (cstart[c + 1] <= cstart[c]) return ra_fail(B200RA_ERR_INPUT, "camera %d: no frames to average over", c);
+      L.cstart[c + 1] = p->cam_frame_start[c + 1];
+      if (L.cstart[c + 1] <= L.cstart[c]) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "camera %d: no frames to average over", c);
     }
-    cfr.assign(p->cam_frames, p->cam_frames + cstart[C]);
-    for (int f : cfr) if (f < 0 || f >= F) return ra_fail(B200RA_ERR_INPUT, "camera frame list: frame %d out of range", f);
+    L.cfr.assign(p->cam_frames, p->cam_frames + L.cstart[C]);
+    for (int f : L.cfr) if (f < 0 || f >= F) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "camera frame list: frame %d out of range", f);
   }
   if (n_xz > B200RA_MAX_AXIS_DIM || n_y > B200RA_MAX_AXIS_DIM)
-    return ra_fail(B200RA_ERR_TOO_LARGE, "axis dimensions %d (x/z) and %d (y): the dense limit is %d (a sparse factorisation is not implemented)",
-                   n_xz, n_y, B200RA_MAX_AXIS_DIM);
-  const int same_y = n_xz == n_y;
-  const int Np_xz = (n_xz + BA_TILE - 1) / BA_TILE * BA_TILE, Np_y = same_y ? 0 : (n_y + BA_TILE - 1) / BA_TILE * BA_TILE;
-  const int nrhs_xz = same_y ? 3 : 2;
-  out->status = B200RA_SUCCESS; out->num_l1_iterations = out->num_irls_iterations = 0;
-  out->n_xz = n_xz; out->n_y = n_y; out->num_residuals = (int)m;
-  out->l1_ms = out->irls_ms = out->build_ms = out->factor_ms = out->solve_ms = 0;
-  if (o->max_num_l1_iterations > 0 && m < np) { out->status = B200RA_UNDERDETERMINED; return 0; }
-  if (o->max_num_l1_iterations == 0 && o->max_num_irls_iterations == 0) return 0;
+    return solver_fail(g_ra_err, B200RA_ERR_TOO_LARGE, "axis dimensions %d (x/z) and %d (y): the dense limit is %d (a sparse factorisation is not implemented)",
+                       n_xz, n_y, B200RA_MAX_AXIS_DIM);
+  L.m = m; L.gauge = gauge; L.gdof = gdof; L.n_xz = n_xz; L.n_y = n_y;
+  L.same_y = n_xz == n_y;
+  L.Np_xz = (n_xz + BA_TILE - 1) / BA_TILE * BA_TILE; L.Np_y = L.same_y ? 0 : (n_y + BA_TILE - 1) / BA_TILE * BA_TILE;
 
   // block -> incident pair slots, in pair order
-  std::vector<int> bstart(nb + 1, 0), bent;
-  std::vector<int> h_f1(P), h_f2(P), h_c1(P), h_c2(P);
-  std::vector<uint8_t> h_pdof(P);
+  L.bstart.assign(nb + 1, 0);
+  L.f1.resize(P); L.f2.resize(P); L.c1.resize(P); L.c2.resize(P); L.pdof.resize(P);
   for (int q = 0; q < P; ++q) {
-    h_f1[q] = p->pair_frame1[q]; h_f2[q] = p->pair_frame2[q];
-    h_c1[q] = p->pair_cam1 && p->pair_cam1[q] >= 0 ? F + p->pair_cam1[q] : -1;
-    h_c2[q] = p->pair_cam2 && p->pair_cam2[q] >= 0 ? F + p->pair_cam2[q] : -1;
-    h_pdof[q] = p->pair_dof[q];
-    const int bl[4] = {h_f1[q], h_f2[q], h_c1[q], h_c2[q]};
-    for (int s = 0; s < 4; ++s) if (bl[s] >= 0) bstart[bl[s] + 1]++;
+    L.f1[q] = p->pair_frame1[q]; L.f2[q] = p->pair_frame2[q];
+    L.c1[q] = p->pair_cam1 && p->pair_cam1[q] >= 0 ? F + p->pair_cam1[q] : -1;
+    L.c2[q] = p->pair_cam2 && p->pair_cam2[q] >= 0 ? F + p->pair_cam2[q] : -1;
+    L.pdof[q] = p->pair_dof[q];
+    const int bl[4] = {L.f1[q], L.f2[q], L.c1[q], L.c2[q]};
+    for (int s = 0; s < 4; ++s) if (bl[s] >= 0) L.bstart[bl[s] + 1]++;
   }
-  for (int b = 0; b < nb; ++b) bstart[b + 1] += bstart[b];
-  bent.resize(std::max(1, bstart[nb]));
-  {
-    std::vector<int> fill(bstart.begin(), bstart.end() - 1);
-    for (int q = 0; q < P; ++q) {
-      const int bl[4] = {h_f1[q], h_f2[q], h_c1[q], h_c2[q]};
-      for (int s = 0; s < 4; ++s) if (bl[s] >= 0) bent[fill[bl[s]]++] = 4 * q + s;
+  for (int b = 0; b < nb; ++b) L.bstart[b + 1] += L.bstart[b];
+  L.bent.assign(std::max(1, L.bstart[nb]), 0);
+  std::vector<int> fill(L.bstart.begin(), L.bstart.end() - 1);
+  for (int q = 0; q < P; ++q) {
+    const int bl[4] = {L.f1[q], L.f2[q], L.c1[q], L.c2[q]};
+    for (int s = 0; s < 4; ++s) if (bl[s] >= 0) L.bent[fill[bl[s]]++] = 4 * q + s;
+  }
+  L.rwrow.assign(m, 1.0); L.rw2.resize(P);
+  L.R.assign(9LL * std::max(P, 1), 0.0); L.ang.assign(std::max(P, 1), 0.0); L.xz.assign(std::max(P, 1), 0.0);
+  for (int q = 0; q < P; ++q) {
+    for (int i = 0; i < L.pdof[q]; ++i) L.rwrow[L.roff[q] + i] = L.rw[q];
+    L.rw2[q] = L.rw[q] * L.rw[q];
+    if (L.pdof[q] == 3) for (int k = 0; k < 9; ++k) L.R[9LL * q + k] = p->pair_R[9LL * q + k];
+    else { L.ang[q] = p->pair_angle[q]; L.xz[q] = p->pair_xz_error[q]; }
+  }
+  return 0;
+}
+
+// One axis matrix, M_xz (x and z, and y too when M_y = M_xz) or M_y, padded to Np, with its factor's scratch and its
+// right-hand sides B.  n = 0: the matrix is not used.
+struct RaAxis {
+  int axis_y, n, Np, nrhs;
+  double *M, *dinv, *B, *W;
+  BaDenseFlag* flag;
+};
+
+// L1 then IRLS on the device state g.  Every method returns 0 or B200RA_ERR_CUDA; a numerical failure ends a phase with
+// out->status set.
+struct RaSolve {
+  const b200ra_options* o;
+  b200ra_summary* out;
+  RaDev g;
+  RaAxis axes[2];   // x/z, y
+  double *rw2, *rwrow, *bv, *z, *u, *dz, *er, *ax, *v, *t1, *t2, *stepsz, *red;
+  int* bad;
+  cudaEvent_t ev[4];   // ev[0], ev[1] bracket a phase; ev[2], ev[3] its builds, factorisations and solves
+  double sums[8];
+
+  // deterministic sum (SOLVER_SUM) or sum of squares (SOLVER_SUM_SQ) of n doubles into sums[slot] (read back by fetch)
+  void dsum(int mode, const double* x, int64_t n, int slot) {
+    solver_sum<RA_RG>(mode, x, nullptr, nullptr, 1, n, red, red + RA_RG + slot);
+  }
+  int fetch(int k) {
+    RA_CHECK(cudaMemcpy(sums, red + RA_RG, sizeof(double) * k, cudaMemcpyDeviceToHost));
+    return 0;
+  }
+  int tic() {
+    RA_CHECK(cudaEventRecord(ev[2]));
+    return 0;
+  }
+  int toc(double* acc) {
+    RA_CHECK(cudaEventRecord(ev[3]));
+    RA_CHECK(cudaEventSynchronize(ev[3]));
+    float t = 0;
+    RA_CHECK(cudaEventElapsedTime(&t, ev[2], ev[3]));
+    *acc += t;
+    return 0;
+  }
+  // build and factor the axis matrices with pair weights w; *ok is false after a failed pivot
+  int build_factor(const double* w, bool* ok) {
+    SOLVER_TRY(tic());
+    for (RaAxis& a : axes) {
+      if (!a.n) continue;
+      RA_CHECK(cudaMemset(a.M, 0, sizeof(double) * (size_t)a.Np * a.Np));
+      k_ra_build<<<grid_blocks(a.n, 128), 128>>>(g, a.axis_y, w, o->ridge_regularization, a.M, a.Np);
+      RA_CHECK(ba_dense_pad_identity(a.M, a.Np, a.n, 0));
     }
+    SOLVER_TRY(toc(&out->build_ms));
+    SOLVER_TRY(tic());
+    const BaDenseFlag clear{0, 0, 0.0};
+    for (RaAxis& a : axes) RA_CHECK(cudaMemcpy(a.flag, &clear, sizeof clear, cudaMemcpyHostToDevice));
+    for (RaAxis& a : axes) if (a.n) RA_CHECK(ba_dense_potrf(a.M, a.Np, a.n, a.n, 0.0, a.dinv, a.flag, 0));
+    SOLVER_TRY(toc(&out->factor_ms));
+    *ok = true;
+    for (RaAxis& a : axes) {
+      BaDenseFlag fl{0, 0, 0.0};
+      RA_CHECK(cudaMemcpy(&fl, a.flag, sizeof fl, cudaMemcpyDeviceToHost));
+      *ok = *ok && !fl.bad;
+    }
+    return 0;
   }
-  std::vector<double> rwrow(m, 1.0), rw2(P), h_R(9LL * std::max(P, 1), 0.0), h_ang(std::max(P, 1), 0.0), h_xz(std::max(P, 1), 0.0);
-  for (int q = 0; q < P; ++q) {
-    for (int i = 0; i < h_pdof[q]; ++i) rwrow[roff[q] + i] = rw[q];
-    rw2[q] = rw[q] * rw[q];
-    if (h_pdof[q] == 3) for (int k = 0; k < 9; ++k) h_R[9LL * q + k] = p->pair_R[9LL * q + k];
-    else { h_ang[q] = p->pair_angle[q]; h_xz[q] = p->pair_xz_error[q]; }
+  // step (parameter order) = (A^T W A)^-1 rhs (parameter order)
+  int solve(const double* rhs) {
+    SOLVER_TRY(tic());
+    k_ra_scatter<<<grid_blocks(g.nb, 128), 128>>>(g, rhs, axes[0].B, axes[1].B, 1);
+    for (RaAxis& a : axes) if (a.n) RA_CHECK(ba_dense_potrs(a.M, a.Np, a.dinv, a.nrhs, a.B, a.W, a.flag, 0));
+    k_ra_scatter<<<grid_blocks(g.nb, 128), 128>>>(g, nullptr, axes[0].B, axes[1].B, 0);
+    return toc(&out->solve_ms);
+  }
+  // UpdateState and AverageStepSize
+  int update(double* avg) {
+    k_ra_update_frames<<<grid_blocks(g.F, 128), 128>>>(g, stepsz);
+    if (g.C) k_ra_update_cameras<<<g.C, RA_CB>>>(g);
+    dsum(SOLVER_SUM, stepsz, g.F, 0);
+    SOLVER_TRY(fetch(1));
+    *avg = sums[0] / g.F;
+    return 0;
+  }
+  // end of a phase: its device time into *ms
+  int phase_time(double* ms) {
+    RA_CHECK(cudaEventRecord(ev[1]));
+    RA_CHECK(cudaEventSynchronize(ev[1]));
+    float t = 0;
+    RA_CHECK(cudaEventElapsedTime(&t, ev[0], ev[1]));
+    *ms = t;
+    return 0;
   }
 
-  int rc = 0;
-  if (o->gpu_index >= 0) {
-    int ndev = 0; cudaGetDeviceCount(&ndev);
-    if (o->gpu_index >= ndev) return ra_fail(B200RA_ERR_INPUT, "gpu_index out of range");
-    cudaSetDevice(o->gpu_index);
+  // SolveL1Regression (:704-770)
+  int l1(int* hist) {
+    const int m = g.m, np = g.np;
+    const unsigned pb = grid_blocks((int64_t)g.P + 1, 128), mb = grid_blocks(m, 256), bb = grid_blocks(g.nb, 128);
+    RA_CHECK(cudaEventRecord(ev[0]));
+    bool ok;
+    SOLVER_TRY(build_factor(rw2, &ok));
+    if (!ok) { out->status = B200RA_FACTORIZATION_FAILED; return 0; }
+    double prev_norm = 0, curr_norm = 0;
+    int max_admm = 10;
+    const double eps_pri0 = sqrt((double)m) * B200RA_ADMM_ABS_TOL, eps_dual0 = sqrt((double)np) * B200RA_ADMM_ABS_TOL;
+    int it = 0;
+    for (; it < o->max_num_l1_iterations; ++it) {
+      k_ra_residuals<<<pb, 128>>>(g);
+      k_ra_mul<<<mb, 256>>>(m, rwrow, g.res, bv);
+      RA_CHECK(cudaMemset(z, 0, sizeof(double) * m));
+      RA_CHECK(cudaMemset(u, 0, sizeof(double) * m));
+      dsum(SOLVER_SUM_SQ, bv, m, 0);
+      SOLVER_TRY(fetch(1));
+      const double b_norm = sqrt(sums[0]);
+      int i = 0;
+      for (; i < max_admm; ++i) {
+        k_ra_admm_rhs<<<mb, 256>>>(m, bv, z, u, v);
+        k_ra_atv<<<bb, 128>>>(g, g.rw, v, t1);
+        SOLVER_TRY(solve(t1));
+        k_ra_ax<<<pb, 128>>>(g, g.step, ax);
+        k_ra_admm_rows<<<mb, 256>>>(m, ax, bv, z, u, dz, er);
+        k_ra_atv<<<bb, 128>>>(g, g.rw, dz, t1);
+        k_ra_atv<<<bb, 128>>>(g, g.rw, u, t2);
+        dsum(SOLVER_SUM_SQ, er, m, 0); dsum(SOLVER_SUM_SQ, ax, m, 1); dsum(SOLVER_SUM_SQ, z, m, 2);
+        dsum(SOLVER_SUM_SQ, t1, np, 3); dsum(SOLVER_SUM_SQ, t2, np, 4);
+        SOLVER_TRY(fetch(5));
+        const double r_norm = sqrt(sums[0]);
+        const double s_norm = B200RA_ADMM_RHO * sqrt(sums[3]);
+        const double eps_pri = eps_pri0 + B200RA_ADMM_REL_TOL * std::max(b_norm, std::max(sqrt(sums[1]), sqrt(sums[2])));
+        const double eps_dual = eps_dual0 + B200RA_ADMM_REL_TOL * (B200RA_ADMM_RHO * sqrt(sums[4]));
+        if (r_norm < eps_pri && s_norm < eps_dual) { ++i; break; }
+      }
+      if (out->admm_iterations) out->admm_iterations[it] = i;
+      prev_norm = curr_norm;
+      dsum(SOLVER_SUM_SQ, g.step, np, 0);
+      SOLVER_TRY(fetch(1));
+      curr_norm = sqrt(sums[0]);
+      if (std::isnan(curr_norm)) { out->status = B200RA_NAN_STEP; out->num_l1_iterations = it; return 0; }
+      double avg;
+      SOLVER_TRY(update(&avg));
+      if (out->step_history) out->step_history[*hist] = avg;
+      ++*hist;
+      if (avg < o->l1_step_convergence_threshold || fabs(prev_norm - curr_norm) < 1e-12) { ++it; break; }
+      max_admm = std::min(max_admm * 2, 100);
+    }
+    out->num_l1_iterations = it;
+    return phase_time(&out->l1_ms);
   }
-  RaDev g; memset(&g, 0, sizeof g);
-  g.F = F; g.C = C; g.nb = nb; g.P = P; g.m = (int)m; g.np = np; g.gauge = gauge; g.gdof = gdof; g.same_y = same_y;
-  g.n_xz = n_xz; g.n_y = n_y; g.Np_xz = Np_xz; g.Np_y = Np_y;
+
+  // SolveIRLS (:835-902)
+  int irls(int* hist) {
+    RA_CHECK(cudaEventRecord(ev[0]));
+    const double sigma = o->irls_loss_parameter_sigma * M_PI / 180.0;
+    int it = 0;
+    for (; it < o->max_num_irls_iterations; ++it) {
+      k_ra_residuals<<<grid_blocks((int64_t)g.P + 1, 128), 128>>>(g);
+      int flag = 0;
+      RA_CHECK(cudaMemcpy(bad, &flag, sizeof flag, cudaMemcpyHostToDevice));
+      if (g.P) k_ra_irls_weights<<<grid_blocks(g.P, 128), 128>>>(g, sigma, o->weight_type == B200RA_HALF_NORM, bad);
+      RA_CHECK(cudaMemcpy(&flag, bad, sizeof flag, cudaMemcpyDeviceToHost));
+      if (flag) { out->status = B200RA_NAN_WEIGHT; out->num_irls_iterations = it; return 0; }
+      bool ok;
+      SOLVER_TRY(build_factor(g.w, &ok));
+      if (!ok) { out->status = B200RA_FACTORIZATION_FAILED; out->num_irls_iterations = it; return 0; }
+      k_ra_atv<<<grid_blocks(g.nb, 128), 128>>>(g, g.w, g.res, t1);
+      SOLVER_TRY(solve(t1));
+      dsum(SOLVER_SUM_SQ, g.step, g.np, 0);
+      SOLVER_TRY(fetch(1));
+      if (std::isnan(sums[0])) { out->status = B200RA_NAN_STEP; out->num_irls_iterations = it; return 0; }
+      double avg;
+      SOLVER_TRY(update(&avg));
+      if (out->step_history) out->step_history[*hist] = avg;
+      ++*hist;
+      if (avg < o->irls_step_convergence_threshold) { ++it; break; }
+    }
+    out->num_irls_iterations = it;
+    return phase_time(&out->irls_ms);
+  }
+};
+
+// RaDev's buffers and the axis systems: the layout and the initial rotations uploaded, the work arrays allocated
+static int ra_upload(const b200ra_problem* p, const RaLayout& L, SolverBuffers& pool, RaSolve& s) {
+  RaDev& g = s.g;
+  memset(&g, 0, sizeof g);
+  g.F = L.F; g.C = L.C; g.nb = L.nb; g.P = L.P; g.m = (int)L.m; g.np = L.np; g.gauge = L.gauge; g.gdof = L.gdof;
+  g.same_y = L.same_y; g.n_xz = L.n_xz; g.n_y = L.n_y; g.Np_xz = L.Np_xz; g.Np_y = L.Np_y;
   for (int k = 0; k < 3; ++k) g.g0[k] = p->gauge_rotation[k];
-  std::vector<void*> allocs;
-  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-  double *Mxz = nullptr, *My = nullptr, *dinv_xz = nullptr, *dinv_y = nullptr, *Bxz = nullptr, *Wxz = nullptr, *By = nullptr, *Wy = nullptr;
-  double *d_rw2 = nullptr, *d_rwrow = nullptr, *bv = nullptr, *z = nullptr, *u = nullptr, *dz = nullptr, *er = nullptr, *ax = nullptr, *v = nullptr;
-  double *t1 = nullptr, *t2 = nullptr, *stepsz = nullptr, *red = nullptr;
-  BaDenseFlag *flag_xz = nullptr, *flag_y = nullptr;
-  int* d_bad = nullptr;
-  auto dalloc = [&](size_t bytes) -> void* { void* q = nullptr; if (cudaMalloc(&q, std::max<size_t>(bytes, 8)) != cudaSuccess) return nullptr; allocs.push_back(q); return q; };
-  auto dput = [&](const void* h, size_t bytes) -> void* { void* q = dalloc(bytes); if (q && bytes) cudaMemcpy(q, h, bytes, cudaMemcpyHostToDevice); return q; };
-#define RA_ALLOC(ptr, type, count) do { ptr = (type*)dalloc(sizeof(type) * (size_t)(count)); if (!ptr) { rc = ra_fail(B200RA_ERR_CUDA, "cudaMalloc failed"); goto cleanup; } } while (0)
-#define RA_PUT(ptr, type, vec) do { ptr = (type*)dput((vec).data(), sizeof(type) * (vec).size()); if (!ptr) { rc = ra_fail(B200RA_ERR_CUDA, "cudaMalloc failed"); goto cleanup; } } while (0)
-  {
-    std::vector<double> rot(p->rotations, p->rotations + np);
-    std::vector<int> cs(cstart), cf(cfr.empty() ? std::vector<int>(1, 0) : cfr), xb(xz_blk.empty() ? std::vector<int>(1, 0) : xz_blk);
-    std::vector<int> ro(roff.empty() ? std::vector<int>(1, 0) : roff);
-    std::vector<double> rwp(rw.empty() ? std::vector<double>(1, 1.0) : rw);
-    RA_PUT(g.off, const int, off); RA_PUT(g.dof, const int, dof); RA_PUT(g.cx, const int, cx); RA_PUT(g.xz_blk, const int, xb);
-    RA_PUT(g.f1, const int, h_f1); RA_PUT(g.f2, const int, h_f2); RA_PUT(g.c1, const int, h_c1); RA_PUT(g.c2, const int, h_c2);
-    RA_PUT(g.roff, const int, ro); RA_PUT(g.pdof, const uint8_t, h_pdof);
-    RA_PUT(g.R12, const double, h_R); RA_PUT(g.ang, const double, h_ang); RA_PUT(g.xz, const double, h_xz);
-    RA_PUT(g.rw, const double, rwp); RA_PUT(g.rwrow, const double, rwrow); RA_PUT(d_rw2, double, rw2);
-    RA_PUT(g.bstart, const int, bstart); RA_PUT(g.bent, const int, bent);
-    RA_PUT(g.cstart, const int, cs); RA_PUT(g.cfr, const int, cf);
-    RA_PUT(g.rot, double, rot);
-    d_rwrow = (double*)g.rwrow;
+  const std::vector<double> rot(p->rotations, p->rotations + L.np);
+  RA_CHECK(pool.upload(&g.off, L.off)); RA_CHECK(pool.upload(&g.dof, L.dof)); RA_CHECK(pool.upload(&g.cx, L.cx));
+  RA_CHECK(pool.upload(&g.xz_blk, L.xz_blk));
+  RA_CHECK(pool.upload(&g.f1, L.f1)); RA_CHECK(pool.upload(&g.f2, L.f2)); RA_CHECK(pool.upload(&g.c1, L.c1));
+  RA_CHECK(pool.upload(&g.c2, L.c2));
+  RA_CHECK(pool.upload(&g.roff, L.roff)); RA_CHECK(pool.upload(&g.pdof, L.pdof));
+  RA_CHECK(pool.upload(&g.R12, L.R)); RA_CHECK(pool.upload(&g.ang, L.ang)); RA_CHECK(pool.upload(&g.xz, L.xz));
+  RA_CHECK(pool.upload(&g.rw, L.rw)); RA_CHECK(pool.upload(&s.rwrow, L.rwrow)); RA_CHECK(pool.upload(&s.rw2, L.rw2));
+  g.rwrow = s.rwrow;
+  RA_CHECK(pool.upload(&g.bstart, L.bstart)); RA_CHECK(pool.upload(&g.bent, L.bent));
+  RA_CHECK(pool.upload(&g.cstart, L.cstart)); RA_CHECK(pool.upload(&g.cfr, L.cfr));
+  RA_CHECK(pool.upload(&g.rot, rot));
+  const int64_t m = L.m;
+  RA_CHECK(pool.alloc(&g.step, L.np)); RA_CHECK(pool.alloc(&g.res, m)); RA_CHECK(pool.alloc(&g.w, std::max(L.P, 1)));
+  RA_CHECK(pool.alloc(&s.bv, m)); RA_CHECK(pool.alloc(&s.z, m)); RA_CHECK(pool.alloc(&s.u, m)); RA_CHECK(pool.alloc(&s.dz, m));
+  RA_CHECK(pool.alloc(&s.er, m)); RA_CHECK(pool.alloc(&s.ax, m)); RA_CHECK(pool.alloc(&s.v, m)); RA_CHECK(pool.alloc(&s.t1, L.np));
+  RA_CHECK(pool.alloc(&s.t2, L.np)); RA_CHECK(pool.alloc(&s.stepsz, L.F)); RA_CHECK(pool.alloc(&s.red, RA_RG + 16));
+  RA_CHECK(pool.alloc(&s.bad, 1));
+  s.axes[0] = RaAxis{0, L.n_xz, L.Np_xz, L.same_y ? 3 : 2};
+  s.axes[1] = RaAxis{1, L.same_y ? 0 : L.n_y, L.Np_y, 1};
+  for (RaAxis& a : s.axes) RA_CHECK(pool.alloc(&a.flag, 1));
+  for (RaAxis& a : s.axes) {
+    if (!a.n) continue;
+    RA_CHECK(pool.alloc(&a.M, (size_t)a.Np * a.Np)); RA_CHECK(pool.alloc(&a.dinv, (size_t)a.Np * BA_TILE));
+    RA_CHECK(pool.alloc(&a.B, (size_t)a.Np * a.nrhs)); RA_CHECK(pool.alloc(&a.W, (size_t)a.Np * a.nrhs));
+    RA_CHECK(cudaMemset(a.B, 0, sizeof(double) * (size_t)a.Np * a.nrhs));
   }
-  RA_ALLOC(g.step, double, np); RA_ALLOC(g.res, double, m); RA_ALLOC(g.w, double, std::max(P, 1));
-  RA_ALLOC(bv, double, m); RA_ALLOC(z, double, m); RA_ALLOC(u, double, m); RA_ALLOC(dz, double, m); RA_ALLOC(er, double, m);
-  RA_ALLOC(ax, double, m); RA_ALLOC(v, double, m); RA_ALLOC(t1, double, np); RA_ALLOC(t2, double, np);
-  RA_ALLOC(stepsz, double, F); RA_ALLOC(red, double, RA_RG + 16); RA_ALLOC(d_bad, int, 1);
-  RA_ALLOC(flag_xz, BaDenseFlag, 1); RA_ALLOC(flag_y, BaDenseFlag, 1);
-  if (n_xz) {
-    RA_ALLOC(Mxz, double, (size_t)Np_xz * Np_xz); RA_ALLOC(dinv_xz, double, (size_t)Np_xz * BA_TILE);
-    RA_ALLOC(Bxz, double, (size_t)Np_xz * nrhs_xz); RA_ALLOC(Wxz, double, (size_t)Np_xz * nrhs_xz);
-    RA_CUDA(cudaMemset(Bxz, 0, sizeof(double) * (size_t)Np_xz * nrhs_xz));
+  for (cudaEvent_t& ev : s.ev) RA_CHECK(pool.event(&ev));
+  return 0;
+}
+
+extern "C" int b200ra_solve(const b200ra_options* o, b200ra_problem* p, b200ra_summary* out) {
+  g_ra_err.clear();
+  if (!o || !p || !out) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "null argument");
+  RaLayout L;
+  SOLVER_TRY(ra_layout(o, p, L));
+  out->status = B200RA_SUCCESS; out->num_l1_iterations = out->num_irls_iterations = 0;
+  out->n_xz = L.n_xz; out->n_y = L.n_y; out->num_residuals = (int)L.m;
+  out->l1_ms = out->irls_ms = out->build_ms = out->factor_ms = out->solve_ms = 0;
+  if (o->max_num_l1_iterations > 0 && L.m < L.np) { out->status = B200RA_UNDERDETERMINED; return 0; }
+  if (o->max_num_l1_iterations == 0 && o->max_num_irls_iterations == 0) return 0;
+
+  if (o->gpu_index >= 0) {
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess) ndev = 0;   // no usable device: the index is out of range
+    if (o->gpu_index >= ndev) return solver_fail(g_ra_err, B200RA_ERR_INPUT, "gpu_index out of range");
+    RA_CHECK(cudaSetDevice(o->gpu_index));
   }
-  if (!same_y) {
-    RA_ALLOC(My, double, (size_t)Np_y * Np_y); RA_ALLOC(dinv_y, double, (size_t)Np_y * BA_TILE);
-    RA_ALLOC(By, double, Np_y); RA_ALLOC(Wy, double, Np_y);
-    RA_CUDA(cudaMemset(By, 0, sizeof(double) * Np_y));
-  }
-  for (int k = 0; k < 4; ++k) RA_CUDA(cudaEventCreate(&ev[k]));
-  {
-    double sums[8];
-    // deterministic sum (mode 0) or sum of squares (mode 1) of n doubles into sums[slot] (read back by fetch())
-    auto dsum = [&](const double* x, int64_t n, int mode, int slot) {
-      k_ra_reduce1<<<RA_RG, RA_RB>>>(x, n, mode, red);
-      k_ra_reduce2<<<1, RA_RG>>>(red, red + RA_RG + slot);
-    };
-    auto fetch = [&](int k) -> cudaError_t { return cudaMemcpy(sums, red + RA_RG, sizeof(double) * k, cudaMemcpyDeviceToHost); };
-    float ms = 0;
-    // timed section helpers: ev[2], ev[3] bracket build / factor / solve pieces
-    auto tic = [&]() { cudaEventRecord(ev[2]); };
-    auto toc = [&](double* acc) { cudaEventRecord(ev[3]); cudaEventSynchronize(ev[3]); float t = 0; cudaEventElapsedTime(&t, ev[2], ev[3]); *acc += t; };
-    // build and factor the axis matrices with pair weights w; false on a failed pivot
-    auto build_factor = [&](const double* w) -> int {
-      tic();
-      if (n_xz) {
-        cudaMemset(Mxz, 0, sizeof(double) * (size_t)Np_xz * Np_xz);
-        k_ra_build<<<ra_blocks(n_xz, 128), 128>>>(g, 0, w, o->ridge_regularization, Mxz, Np_xz);
-        if (Np_xz > n_xz) k_ra_pad_identity<<<ra_blocks(Np_xz - n_xz, 64), 64>>>(Mxz, n_xz, Np_xz);
-      }
-      if (!same_y) {
-        cudaMemset(My, 0, sizeof(double) * (size_t)Np_y * Np_y);
-        k_ra_build<<<ra_blocks(n_y, 128), 128>>>(g, 1, w, o->ridge_regularization, My, Np_y);
-        if (Np_y > n_y) k_ra_pad_identity<<<ra_blocks(Np_y - n_y, 64), 64>>>(My, n_y, Np_y);
-      }
-      toc(&out->build_ms);
-      tic();
-      BaDenseFlag fl{0, 0, 0.0};
-      cudaMemcpy(flag_xz, &fl, sizeof fl, cudaMemcpyHostToDevice);
-      cudaMemcpy(flag_y, &fl, sizeof fl, cudaMemcpyHostToDevice);
-      if (n_xz) ba_dense_potrf(Mxz, Np_xz, n_xz, n_xz, 0.0, dinv_xz, flag_xz, 0);
-      if (!same_y) ba_dense_potrf(My, Np_y, n_y, n_y, 0.0, dinv_y, flag_y, 0);
-      toc(&out->factor_ms);
-      BaDenseFlag a{0, 0, 0.0}, b{0, 0, 0.0};
-      cudaMemcpy(&a, flag_xz, sizeof a, cudaMemcpyDeviceToHost);
-      cudaMemcpy(&b, flag_y, sizeof b, cudaMemcpyDeviceToHost);
-      return !a.bad && !b.bad;
-    };
-    // step (parameter order) = (A^T W A)^-1 rhs (parameter order)
-    auto solve = [&](const double* rhs) {
-      tic();
-      k_ra_scatter<<<ra_blocks(nb, 128), 128>>>(g, rhs, Bxz, By, 1);
-      if (n_xz) ba_dense_potrs(Mxz, Np_xz, dinv_xz, nrhs_xz, Bxz, Wxz, flag_xz, 0);
-      if (!same_y) ba_dense_potrs(My, Np_y, dinv_y, 1, By, Wy, flag_y, 0);
-      k_ra_scatter<<<ra_blocks(nb, 128), 128>>>(g, nullptr, Bxz, By, 0);
-      toc(&out->solve_ms);
-    };
-    // UpdateState and AverageStepSize; returns the average step
-    auto update = [&]() -> double {
-      k_ra_update_frames<<<ra_blocks(F, 128), 128>>>(g, stepsz);
-      if (C) k_ra_update_cameras<<<C, RA_CB>>>(g);
-      dsum(stepsz, F, 0, 0);
-      fetch(1);
-      return sums[0] / F;
-    };
-    const unsigned pb = ra_blocks((int64_t)P + 1, 128), mb = ra_blocks(m, 256);
-    int hist = 0;
-    // ---------------- L1 (SolveL1Regression, :704-770)
-    if (o->max_num_l1_iterations > 0) {
-      RA_CUDA(cudaEventRecord(ev[0]));
-      if (!build_factor(d_rw2)) { out->status = B200RA_FACTORIZATION_FAILED; goto done; }
-      double prev_norm = 0, curr_norm = 0;
-      int max_admm = 10;
-      const double eps_pri0 = sqrt((double)m) * B200RA_ADMM_ABS_TOL, eps_dual0 = sqrt((double)np) * B200RA_ADMM_ABS_TOL;
-      int it = 0;
-      for (; it < o->max_num_l1_iterations; ++it) {
-        k_ra_residuals<<<pb, 128>>>(g);
-        k_ra_mul<<<mb, 256>>>((int)m, d_rwrow, g.res, bv);
-        RA_CUDA(cudaMemset(z, 0, sizeof(double) * m));
-        RA_CUDA(cudaMemset(u, 0, sizeof(double) * m));
-        dsum(bv, m, 1, 0);
-        RA_CUDA(fetch(1));
-        const double b_norm = sqrt(sums[0]);
-        int i = 0;
-        for (; i < max_admm; ++i) {
-          k_ra_admm_rhs<<<mb, 256>>>((int)m, bv, z, u, v);
-          k_ra_atv<<<ra_blocks(nb, 128), 128>>>(g, g.rw, v, t1);
-          solve(t1);
-          k_ra_ax<<<pb, 128>>>(g, g.step, ax);
-          k_ra_admm_rows<<<mb, 256>>>((int)m, ax, bv, z, u, dz, er);
-          k_ra_atv<<<ra_blocks(nb, 128), 128>>>(g, g.rw, dz, t1);
-          k_ra_atv<<<ra_blocks(nb, 128), 128>>>(g, g.rw, u, t2);
-          dsum(er, m, 1, 0); dsum(ax, m, 1, 1); dsum(z, m, 1, 2); dsum(t1, np, 1, 3); dsum(t2, np, 1, 4);
-          RA_CUDA(fetch(5));
-          const double r_norm = sqrt(sums[0]);
-          const double s_norm = B200RA_ADMM_RHO * sqrt(sums[3]);
-          const double eps_pri = eps_pri0 + B200RA_ADMM_REL_TOL * std::max(b_norm, std::max(sqrt(sums[1]), sqrt(sums[2])));
-          const double eps_dual = eps_dual0 + B200RA_ADMM_REL_TOL * (B200RA_ADMM_RHO * sqrt(sums[4]));
-          if (r_norm < eps_pri && s_norm < eps_dual) { ++i; break; }
-        }
-        if (out->admm_iterations) out->admm_iterations[it] = i;
-        prev_norm = curr_norm;
-        dsum(g.step, np, 1, 0);
-        RA_CUDA(fetch(1));
-        curr_norm = sqrt(sums[0]);
-        if (std::isnan(curr_norm)) { out->status = B200RA_NAN_STEP; out->num_l1_iterations = it; goto done; }
-        const double avg = update();
-        if (out->step_history) out->step_history[hist] = avg;
-        ++hist;
-        if (avg < o->l1_step_convergence_threshold || fabs(prev_norm - curr_norm) < 1e-12) { ++it; break; }
-        max_admm = std::min(max_admm * 2, 100);
-      }
-      out->num_l1_iterations = it;
-      RA_CUDA(cudaEventRecord(ev[1])); RA_CUDA(cudaEventSynchronize(ev[1]));
-      cudaEventElapsedTime(&ms, ev[0], ev[1]); out->l1_ms = ms;
-    }
-    // ---------------- IRLS (SolveIRLS, :835-902)
-    if (o->max_num_irls_iterations > 0) {
-      RA_CUDA(cudaEventRecord(ev[0]));
-      const double sigma = o->irls_loss_parameter_sigma * M_PI / 180.0;
-      int it = 0;
-      for (; it < o->max_num_irls_iterations; ++it) {
-        k_ra_residuals<<<pb, 128>>>(g);
-        int zero = 0;
-        RA_CUDA(cudaMemcpy(d_bad, &zero, sizeof zero, cudaMemcpyHostToDevice));
-        if (P) k_ra_irls_weights<<<ra_blocks(P, 128), 128>>>(g, sigma, o->weight_type == B200RA_HALF_NORM, d_bad);
-        int bad = 0;
-        RA_CUDA(cudaMemcpy(&bad, d_bad, sizeof bad, cudaMemcpyDeviceToHost));
-        if (bad) { out->status = B200RA_NAN_WEIGHT; out->num_irls_iterations = it; goto done; }
-        if (!build_factor(g.w)) { out->status = B200RA_FACTORIZATION_FAILED; out->num_irls_iterations = it; goto done; }
-        k_ra_atv<<<ra_blocks(nb, 128), 128>>>(g, g.w, g.res, t1);
-        solve(t1);
-        dsum(g.step, np, 1, 0);
-        RA_CUDA(fetch(1));
-        if (std::isnan(sums[0])) { out->status = B200RA_NAN_STEP; out->num_irls_iterations = it; goto done; }
-        const double avg = update();
-        if (out->step_history) out->step_history[hist] = avg;
-        ++hist;
-        if (avg < o->irls_step_convergence_threshold) { ++it; break; }
-      }
-      out->num_irls_iterations = it;
-      RA_CUDA(cudaEventRecord(ev[1])); RA_CUDA(cudaEventSynchronize(ev[1]));
-      cudaEventElapsedTime(&ms, ev[0], ev[1]); out->irls_ms = ms;
-    }
-  done:
-    RA_CUDA(cudaGetLastError());
-    RA_CUDA(cudaDeviceSynchronize());
-    if (out->status == B200RA_SUCCESS) RA_CUDA(cudaMemcpy(p->rotations, g.rot, sizeof(double) * np, cudaMemcpyDeviceToHost));
-  }
-cleanup:
-  for (void* q : allocs) cudaFree(q);
-  for (int k = 0; k < 4; ++k) if (ev[k]) cudaEventDestroy(ev[k]);
-  return rc;
+  SolverBuffers pool;
+  RaSolve s{o, out};
+  SOLVER_TRY(ra_upload(p, L, pool, s));
+  int hist = 0;
+  if (o->max_num_l1_iterations > 0) SOLVER_TRY(s.l1(&hist));
+  if (out->status == B200RA_SUCCESS && o->max_num_irls_iterations > 0) SOLVER_TRY(s.irls(&hist));
+  RA_CHECK(cudaGetLastError());
+  RA_CHECK(cudaDeviceSynchronize());
+  if (out->status == B200RA_SUCCESS) RA_CHECK(cudaMemcpy(p->rotations, s.g.rot, sizeof(double) * L.np, cudaMemcpyDeviceToHost));
+  return 0;
 }
