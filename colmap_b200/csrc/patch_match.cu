@@ -76,7 +76,6 @@ struct PmSweepArgs {
   const float* sel_prev;
   // split pipeline scratch (per pixel, original-orientation pixel index)
   float4* rand_hyp;        // random hypothesis of the pixel in the sweep frame {depth, n}
-  unsigned char* ntrials;  // PerturbNormal rounds consumed (each 3 draws)
   float* usamp;            // [pixel][num_samples] Monte-Carlo uniforms (already minus FLT_EPSILON, :1129)
   float* prior3;           // [pixel][3][N] triangulation / incident / resolution priors of the current hypothesis
   float* tab3;             // [pixel][3][N] NCC of hypotheses 2,3,4 for every source image
@@ -95,7 +94,7 @@ struct PmSweepArgs {
 // frame maps: frame k = the reference's buffers after k Rotate() calls (cuda_rotate.h:57-75):
 //   (r_{k+1}, c_{k+1}) = (w_k - 1 - c_k, r_k)
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void pm_frame_to_orig(int W0, int H0, int rot, int r, int c, int* r0, int* c0) {
+__host__ __device__ __forceinline__ void pm_frame_to_orig(int W0, int H0, int rot, int r, int c, int* r0, int* c0) {
   switch (rot) {
     case 0: *r0 = r; *c0 = c; break;
     case 1: *r0 = c; *c0 = W0 - 1 - r; break;
@@ -104,14 +103,14 @@ __device__ __forceinline__ void pm_frame_to_orig(int W0, int H0, int rot, int r,
   }
 }
 // The four frame maps are affine in (r, c): pixel index = base + r * stride_r + c * stride_c (two IMADs, no branch)
-__device__ __forceinline__ size_t pm_pix0(int W0, int H0, int rot, int r, int c) {
+__host__ __device__ __forceinline__ size_t pm_pix0(int W0, int H0, int rot, int r, int c) {
   const int sr = (rot == 0) ? W0 : ((rot == 1) ? -1 : ((rot == 2) ? -W0 : 1));
   const int sc = (rot == 0) ? 1 : ((rot == 1) ? W0 : ((rot == 2) ? -1 : -W0));
   const int base = (rot == 0) ? 0 : ((rot == 1) ? (W0 - 1) : ((rot == 2) ? (H0 * W0 - 1) : ((H0 - 1) * W0)));
   return (size_t)(base + r * sr + c * sc);
 }
 // RotateNormalMap applied k times / undone (patch_match_cuda.cu:849-861)
-__device__ __forceinline__ void pm_normal_to_frame(int rot, float& nx, float& ny) {
+__host__ __device__ __forceinline__ void pm_normal_to_frame(int rot, float& nx, float& ny) {
   const float x = nx, y = ny;
   switch (rot) {
     case 0: break;
@@ -543,8 +542,8 @@ __global__ void __launch_bounds__(128) pm_initial_cost_kernel(const PmParams P) 
 
 // ================================================================================================
 // Sweep: SweepFromTopToBottom (patch_match_cuda.cu:933-1288) in four passes.
-//   R  pm_rand_kernel    column-serial, one thread per column: consumes the column's XORWOW stream to
-//                        produce every row's random hypothesis (the stream position of a row does not
+//   R  pm_rand_kernel    one warp per column: consumes the column's XORWOW stream to produce every row's
+//                        random hypothesis and Monte-Carlo uniforms (the stream position of a row does not
 //                        depend on the sweep's results, only on the hypotheses of the previous sweep);
 //   M  pm_msg_kernel     one thread per (column, image), beside R: the column's HMM messages over the
 //                        costs the sweep starts with;
@@ -555,70 +554,164 @@ __global__ void __launch_bounds__(128) pm_initial_cost_kernel(const PmParams P) 
 //   S  pm_serial_kernel  one CTA per column: propagation, HMM messages, Monte-Carlo sampling, the NCC
 //                        of the propagated hypothesis, argmin, filter.
 // ================================================================================================
-__global__ void pm_rand_kernel(const PmParams P, const PmSweepArgs A) {
-  const int rot = A.rot;
-  const int fw = (rot & 1) ? P.H0 : P.W0, fh = (rot & 1) ? P.W0 : P.H0;
-  const int col = blockIdx.x * blockDim.x + threadIdx.x;
-  if (col >= fw) return;
-  const float iK[4] = {P.invK[rot][0], P.invK[rot][1], P.invK[rot][2], P.invK[rot][3]};
-  int r0, c0;
-  pm_frame_to_orig(P.W0, P.H0, rot, 0, col, &r0, &c0);
-  const uint32_t* slot = P.rng + 6 * (size_t)pm_border_index(P.W0, P.H0, r0, c0);
-  PmRng rs;
-  rs.v0 = slot[0]; rs.v1 = slot[1]; rs.v2 = slot[2]; rs.v3 = slot[3]; rs.v4 = slot[4]; rs.d = slot[5];
-  const float colf = (float)col;
-  size_t p = pm_pix0(P.W0, P.H0, rot, 0, col);
-  float4 cur4 = P.hyp[p];
-  for (int row = 0; row < fh; ++row) {
-    const size_t pn = (row + 1 < fh) ? pm_pix0(P.W0, P.H0, rot, row + 1, col) : p;
-    const float4 next4 = P.hyp[pn];  // prefetch the next row while this one is processed
-    float n0 = cur4.y, n1 = cur4.z;
-    pm_normal_to_frame(rot, n0, n1);
-    const float dmin = (1.0f - A.perturbation) * cur4.x;
-    const float dmax = (1.0f + A.perturbation) * cur4.x;
-    const float rand_d = fmaf(pm_rng_uniform(rs), dmax - dmin, dmin);
-    float rn[3];
-    const int rounds = pm_perturb_normal(iK, (float)row, colf, A.perturbation_pi, n0, n1, cur4.w, rs, rn);
-    A.rand_hyp[p] = make_float4(rand_d, rn[0], rn[1], rn[2]);
-    A.ntrials[p] = (unsigned char)rounds;
-    for (int s = 0; s < P.num_samples; ++s) A.usamp[p * P.num_samples + s] = pm_rng_uniform(rs) - FLT_EPSILON;
-    p = pn; cur4 = next4;
-  }
-  uint32_t* wslot = P.rng + 6 * (size_t)pm_border_index(P.W0, P.H0, r0, c0);
-  wslot[0] = rs.v0; wslot[1] = rs.v1; wslot[2] = rs.v2; wslot[3] = rs.v3; wslot[4] = rs.v4; wslot[5] = rs.d;
+// pixel-index step from row r to row r + 1 of frame `rot` (the row stride of pm_pix0)
+__device__ __forceinline__ int pm_row_stride(int W0, int rot) {
+  return (rot == 0) ? W0 : ((rot == 1) ? -1 : ((rot == 2) ? -W0 : 1));
 }
 
+// R  pm_rand_kernel: one warp per PM_RAND_CPW columns.  A row takes 1 + 3 * rounds + num_samples draws from the
+// column's stream, and only `rounds` (PerturbNormal's trials) depends on anything but the stream; that is the only
+// serial part of the pass.  Per block of 32 rows, lane j < PM_RAND_CPW walks column j's stream alone and leaves every
+// row's start state in a shared ring; then lane k restarts from row k's state, column by column, and computes that row
+// with the same functions and draws as a column-serial loop (pm_rand_column_host).  On the tall frames the rows of a
+// column are adjacent pixels, so the 32 lanes' stores are one contiguous run.
+// The walk keeps no results.  A trial's draws are the same whether it is accepted or not, so the walk advances a copy
+// of the stream past the row's sample draws while the trial's acceptance test is computed, and keeps that copy when the
+// trial ends the row; with NS = num_samples known at compile time the two are one straight block the scheduler
+// interleaves (NS = 0: num_samples read at run time, for the configurations other than the default 15).
+#define PM_RAND_WARPS 2   // warps per CTA
+#define PM_RAND_CPW 4     // columns per warp
+template <int NS>
+__global__ void __launch_bounds__(32 * PM_RAND_WARPS) pm_rand_kernel(const PmParams P, const PmSweepArgs A) {
+  constexpr int CPW = PM_RAND_CPW;
+  __shared__ uint32_t ring[PM_RAND_WARPS][CPW][6][32];   // [column][state word][row of the block]
+  __shared__ float4 hyr[PM_RAND_WARPS][CPW][32];         // the block's current hypotheses, for the walks' trials
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int rot = A.rot;
+  const int fw = (rot & 1) ? P.H0 : P.W0, fh = (rot & 1) ? P.W0 : P.H0;
+  const int col0 = (blockIdx.x * PM_RAND_WARPS + warp) * CPW;
+  if (col0 >= fw) return;
+  const int ncols = min(CPW, fw - col0);
+  const float iK[4] = {P.invK[rot][0], P.invK[rot][1], P.invK[rot][2], P.invK[rot][3]};
+  const int ns = NS ? NS : P.num_samples;
+  const bool walker = lane < ncols;
+  const int wcol = col0 + (walker ? lane : 0);   // the column lane `lane` walks
+  int r0, c0;
+  pm_frame_to_orig(P.W0, P.H0, rot, 0, wcol, &r0, &c0);
+  uint32_t* slot = P.rng + 6 * (size_t)pm_border_index(P.W0, P.H0, r0, c0);
+  PmRng rs;
+  if (walker) { rs.v0 = slot[0]; rs.v1 = slot[1]; rs.v2 = slot[2]; rs.v3 = slot[3]; rs.v4 = slot[4]; rs.d = slot[5]; }
+  const long long rstep = pm_row_stride(P.W0, rot);
+  const long long cstep = (long long)pm_pix0(P.W0, P.H0, rot, 0, 1) - (long long)pm_pix0(P.W0, P.H0, rot, 0, 0);
+  const size_t p_top = pm_pix0(P.W0, P.H0, rot, 0, col0);   // column col0 + j, row r: p_top + j * cstep + r * rstep
+  float4 nx[CPW];
+#pragma unroll
+  for (int j = 0; j < CPW; ++j)
+    nx[j] = (j < ncols && lane < fh) ? P.hyp[p_top + j * cstep + lane * rstep] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+  for (int base = 0; base < fh; base += 32) {
+    const int row = base + lane;
+    float4 cur[CPW];
+#pragma unroll
+    for (int j = 0; j < CPW; ++j) {
+      cur[j] = nx[j];
+      if (j < ncols && row + 32 < fh) nx[j] = P.hyp[p_top + j * cstep + (row + 32) * rstep];   // next block's, in flight
+      hyr[warp][j][lane] = cur[j];
+    }
+    __syncwarp();
+    if (walker) {
+      const int nrows = min(32, fh - base);
+      const float colf = (float)wcol;
+      const float rx = fmaf(iK[0], colf, iK[1]);   // pm_perturb_normal's viewing ray
+      for (int k = 0; k < nrows; ++k) {
+        ring[warp][lane][0][k] = rs.v0; ring[warp][lane][1][k] = rs.v1; ring[warp][lane][2][k] = rs.v2;
+        ring[warp][lane][3][k] = rs.v3; ring[warp][lane][4][k] = rs.v4; ring[warp][lane][5][k] = rs.d;
+        const float4 h = hyr[warp][lane][k];
+        float n0 = h.y, n1 = h.z;
+        pm_normal_to_frame(rot, n0, n1);
+        const float ry = fmaf(iK[2], (float)(base + k), iK[3]);
+        pm_rng_next(rs);   // the random depth
+        float perturbation = A.perturbation_pi;
+        for (int trial = 0;; ++trial) {
+          const float u1 = pm_rng_uniform(rs);
+          const float u2 = pm_rng_uniform(rs);
+          const float u3 = pm_rng_uniform(rs);
+          PmRng after = rs;   // the stream past the row's sample draws, if this trial ends the row
+          if (NS) {
+#pragma unroll
+            for (int s = 0; s < NS; ++s) pm_rng_next(after);
+          } else {
+            for (int s = 0; s < ns; ++s) pm_rng_next(after);
+          }
+          float out[3];
+          if (pm_perturb_trial(rx, ry, perturbation, u1, u2, u3, n0, n1, h.w, out) || trial == 3) { rs = after; break; }
+          perturbation = 0.5f * perturbation;
+        }
+      }
+    }
+    __syncwarp();
+#pragma unroll
+    for (int j = 0; j < CPW; ++j) {
+      if (j < ncols && row < fh) {
+        PmRng rk;
+        rk.v0 = ring[warp][j][0][lane]; rk.v1 = ring[warp][j][1][lane]; rk.v2 = ring[warp][j][2][lane];
+        rk.v3 = ring[warp][j][3][lane]; rk.v4 = ring[warp][j][4][lane]; rk.d = ring[warp][j][5][lane];
+        const float4 c4 = cur[j];
+        float n0 = c4.y, n1 = c4.z;
+        pm_normal_to_frame(rot, n0, n1);
+        const float dmin = (1.0f - A.perturbation) * c4.x;
+        const float dmax = (1.0f + A.perturbation) * c4.x;
+        const float rand_d = fmaf(pm_rng_uniform(rk), dmax - dmin, dmin);
+        float rn[3];
+        pm_perturb_normal(iK, (float)row, (float)(col0 + j), A.perturbation_pi, n0, n1, c4.w, rk, rn);
+        const size_t p = p_top + j * cstep + row * rstep;
+        A.rand_hyp[p] = make_float4(rand_d, rn[0], rn[1], rn[2]);
+        for (int s = 0; s < ns; ++s) A.usamp[p * ns + s] = pm_rng_uniform(rk) - FLT_EPSILON;
+      }
+    }
+    // (the next block's first __syncwarp orders this block's ring and hyr reads before their next writes)
+  }
+  if (walker) { slot[0] = rs.v0; slot[1] = rs.v1; slot[2] = rs.v2; slot[3] = rs.v3; slot[4] = rs.v4; slot[5] = rs.d; }
+}
 
 // M  pm_msg_kernel: one thread per (column, image).  Backward messages of the whole column (:976-989) - the same
 // recurrence pm_serial_kernel used to run at its start, now available BEFORE the pixel pass - and the forward
 // messages over the sweep-start costs ("nothing above this row changes"), which is what the serial pass will see
 // wherever no new hypothesis won above.  From them the pixel pass predicts the Monte-Carlo samples of every pixel.
-__global__ void pm_msg_kernel(const PmParams P, const PmSweepArgs A) {
+// The two recurrences are independent and run interleaved, step k of both together (backward at row fh - 1 - k,
+// forward at row k).  A step's likelihood pm_ncc_prob(cost) does not depend on the message, so it is computed off the
+// chains, and the costs are read a chunk of PM_MSG_CHUNK rows ahead: the next chunk's loads are in flight while a chunk
+// is consumed.  Per step the messages are the same operations in the same order as pm_msg_column_host.
+#define PM_MSG_CHUNK 16
+#define PM_MSG_THREADS 64
+__global__ void __launch_bounds__(PM_MSG_THREADS) pm_msg_kernel(const PmParams P, const PmSweepArgs A) {
   const int rot = A.rot, N = P.N;
   const int fw = (rot & 1) ? P.H0 : P.W0, fh = (rot & 1) ? P.W0 : P.H0;
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   const int col = t / N, img = t - col * N;
   if (col >= fw) return;
-  float beta = 0.5f;
-  {
-    float cn = P.cost[pm_pix0(P.W0, P.H0, rot, fh - 1, col) * N + img];
-    for (int row = fh - 1; row >= 0; --row) {
-      const size_t p = pm_pix0(P.W0, P.H0, rot, row, col);
-      const float c = cn;
-      if (row > 0) cn = P.cost[pm_pix0(P.W0, P.H0, rot, row - 1, col) * N + img];   // next load in flight during the chain step
-      beta = pm_backward_message(P.L, c, beta);
-      A.sel_cur[p * N + img] = beta;
+  const bool fwd = A.fwd_pred != nullptr;
+  // value (row, img) of a [pixel][N] map is at top + row * rstep
+  const size_t top = pm_pix0(P.W0, P.H0, rot, 0, col) * N + img;
+  const long long rstep = (long long)pm_row_stride(P.W0, rot) * N;
+  const float* cost = P.cost + top;
+  constexpr int C = PM_MSG_CHUNK;
+  float cb[C], cf[C];   // the chunk's costs: backward rows fh - 1 - k, forward rows k
+  auto load = [&](int k0, float* b, float* f) {
+#pragma unroll
+    for (int j = 0; j < C; ++j) {
+      const int k = k0 + j;
+      b[j] = (k < fh) ? cost[(fh - 1 - k) * rstep] : 0.0f;
+      f[j] = (fwd && k < fh) ? cost[k * rstep] : 0.0f;
     }
-  }
-  if (A.fwd_pred == nullptr) return;
-  float f = 0.5f;
-  float cn = P.cost[pm_pix0(P.W0, P.H0, rot, 0, col) * N + img];
-  for (int row = 0; row < fh; ++row) {
-    const size_t p = pm_pix0(P.W0, P.H0, rot, row, col);
-    const float c = cn;
-    if (row + 1 < fh) cn = P.cost[pm_pix0(P.W0, P.H0, rot, row + 1, col) * N + img];
-    f = pm_forward_message(P.L, c, f);
-    A.fwd_pred[p * N + img] = f;
+  };
+  load(0, cb, cf);
+  float beta = 0.5f, f = 0.5f;
+  for (int k0 = 0; k0 < fh; k0 += C) {
+    float eb[C], ef[C];
+#pragma unroll
+    for (int j = 0; j < C; ++j) { eb[j] = pm_ncc_prob(P.L, cb[j]); ef[j] = pm_ncc_prob(P.L, cf[j]); }
+    load(k0 + C, cb, cf);
+#pragma unroll
+    for (int j = 0; j < C; ++j) {
+      const int k = k0 + j;
+      if (k >= fh) break;
+      beta = pm_backward_message_e(eb[j], beta);
+      A.sel_cur[top + (fh - 1 - k) * rstep] = beta;
+      if (fwd) {
+        f = pm_forward_message_e(ef[j], f);
+        A.fwd_pred[top + k * rstep] = f;
+      }
+    }
   }
 }
 
@@ -1407,6 +1500,8 @@ static int pm_fail(int code, const std::string& msg) { g_pm_error = msg; return 
       return pm_fail(-100, std::string(#call) + ": " + cudaGetErrorString(e__));                  \
   } while (0)
 
+#define PM_NUM_PASS_TIMES 5   // b200pm_last_pass_ms indices: R|M, P, S, R alone, M alone
+
 struct b200pm_context {
   b200pm_options opt;
   PmParams P;
@@ -1424,15 +1519,18 @@ struct b200pm_context {
   int final_sel = 0;
   bool dirty = false, ran = false;
   float last_ms = 0.0f, last_sweep_ms = 0.0f;
-  float last_kernel_ms[3] = {0.0f, 0.0f, 0.0f};  // rand(+msg) / pixel / serial passes of the last run
-  std::vector<float> last_sweep_pass_ms;          // the same per sweep: [sweep][3]
-  std::vector<cudaEvent_t> sweep_ev;
+  // rand(+msg) / pixel / serial passes of the last run, then rand and msg alone (b200pm_last_pass_ms)
+  float last_kernel_ms[PM_NUM_PASS_TIMES] = {};
+  std::vector<float> last_sweep_pass_ms;          // the same per sweep: [sweep][PM_NUM_PASS_TIMES]
+  std::vector<cudaEvent_t> sweep_ev;              // [sweep][4] on the main stream: start, R|M done, P done, S done
+  std::vector<cudaEvent_t> rm_ev;                 // [sweep][3]: R done (main stream), M start and M done (stream2)
   int last_launches = 0;
   std::vector<int> src_image_idxs;
   size_t smem_init = 0, smem_serial = 0, smem_patch = 0;
   size_t smem_pixel4 = 0;   // 0: the pixel pass runs pm_pixel_kernel (N > 8, or four split patches do not fit a CTA)
   size_t patch_store_bytes = 0;   // 0: the reference patches are built inline by every consumer
-  float4* rand_hyp = nullptr; unsigned char* ntrials = nullptr; float* usamp = nullptr; float* prior3 = nullptr; float* tab3 = nullptr; float* gtab2 = nullptr;
+  int last_sweeps = 0;      // sweeps the last run did (B200PM_MAX_SWEEPS can stop it early)
+  float4* rand_hyp = nullptr; float* usamp = nullptr; float* prior3 = nullptr; float* tab3 = nullptr; float* gtab2 = nullptr;
   float* fwd_pred = nullptr;
 };
 // pixels a pixel-pass warp handles before its CTA retires (4 measured fastest on the H100; 8 was ~7 ms per C2 run slower)
@@ -1712,7 +1810,6 @@ int b200pm_create(const b200pm_options* o, const b200pm_problem* p, b200pm_handl
     c->patch_store_bytes = store_bytes;
   }
   PM_CUDA(pm_alloc(c, &c->rand_hyp, n));
-  PM_CUDA(pm_alloc(c, &c->ntrials, n));
   PM_CUDA(pm_alloc(c, &c->usamp, n * (size_t)o->num_samples));
   PM_CUDA(pm_alloc(c, &c->prior3, 3 * n * N));
   PM_CUDA(pm_alloc(c, &c->tab3, 3 * n * N));
@@ -1741,6 +1838,43 @@ template <int WPC>
 static void pm_launch_serial(b200pm_context* c, const PmSweepArgs& A, int fw) {
   if (c->P.patch_store) pm_launch_serial_store<WPC, true>(c, A, fw);
   else pm_launch_serial_store<WPC, false>(c, A, fw);
+}
+
+// The arguments of sweep t (iteration t / 4, frame t % 4) of a run
+static PmSweepArgs pm_sweep_args(const b200pm_context* c, int t) {
+  const int iters = c->opt.num_iterations, iter = t / 4, sweep = t % 4;
+  const float total_steps = (float)(iters * 4);
+  PmSweepArgs A;
+  memset(&A, 0, sizeof(A));
+  A.rot = sweep;
+  A.perturbation = 1.0f / powf(2.0f, (float)iter + (float)sweep / 4.0f);
+  A.perturbation_pi = (float)((double)A.perturbation * M_PI);
+  A.prev_w = (float)(iter * 4 + sweep) / total_steps;
+  A.last_filter = (iter == iters - 1 && sweep == 3 && c->opt.filter) ? 1 : 0;
+  A.sel_cur = c->sel[t & 1];
+  A.sel_prev = c->sel[(t + 1) & 1];
+  A.rand_hyp = c->rand_hyp; A.usamp = c->usamp; A.prior3 = c->prior3; A.tab3 = c->tab3; A.gtab2 = c->gtab2;
+  A.fwd_pred = c->fwd_pred;
+  A.prune = (c->prune == 1) ? ((t >= c->prune_from) ? 1 : 0) : c->prune;
+  return A;
+}
+
+// Pass M (messages) on stream2 beside pass R (random hypotheses) on the main stream: both only read the state the last
+// sweep left.  The main stream goes on when both are done.  ev: nullptr, or the sweep's timing events {R done, M start,
+// M done}.
+static void pm_launch_rand_msg(b200pm_context* c, const PmSweepArgs& A, const cudaEvent_t* ev) {
+  const int fw = (A.rot & 1) ? c->P.H0 : c->P.W0;
+  cudaEventRecord(c->fork_ev, c->stream);
+  cudaStreamWaitEvent(c->stream2, c->fork_ev, 0);
+  if (ev) cudaEventRecord(ev[1], c->stream2);
+  pm_msg_kernel<<<(fw * c->P.N + PM_MSG_THREADS - 1) / PM_MSG_THREADS, PM_MSG_THREADS, 0, c->stream2>>>(c->P, A);
+  if (ev) cudaEventRecord(ev[2], c->stream2);
+  cudaEventRecord(c->join_ev, c->stream2);
+  const int rgrid = (fw + PM_RAND_WARPS * PM_RAND_CPW - 1) / (PM_RAND_WARPS * PM_RAND_CPW);
+  if (c->P.num_samples == 15) pm_rand_kernel<15><<<rgrid, 32 * PM_RAND_WARPS, 0, c->stream>>>(c->P, A);
+  else pm_rand_kernel<0><<<rgrid, 32 * PM_RAND_WARPS, 0, c->stream>>>(c->P, A);
+  if (ev) cudaEventRecord(ev[0], c->stream);
+  cudaStreamWaitEvent(c->stream, c->join_ev, 0);
 }
 
 extern "C" {
@@ -1786,39 +1920,22 @@ int b200pm_run(b200pm_handle c) {
   }
   PM_CUDA(cudaEventRecord(c->ev[1], s));
   const int iters = c->opt.num_iterations;
-  const float total_steps = (float)(iters * 4);
   int t = 0;
   const int max_sweeps = getenv("B200PM_MAX_SWEEPS") ? atoi(getenv("B200PM_MAX_SWEEPS")) : -1;
   c->final_sel = 1;   // until a sweep runs, the selection probability is the 0.5 that pm_init_kernel wrote to sel[1]
   for (int iter = 0; iter < iters; ++iter) {
     for (int sweep = 0; sweep < 4; ++sweep, ++t) {
       if (max_sweeps >= 0 && t >= max_sweeps) break;
-      PmSweepArgs A;
-      memset(&A, 0, sizeof(A));
-      A.rot = sweep;
-      A.perturbation = 1.0f / powf(2.0f, (float)iter + (float)sweep / 4.0f);
-      A.perturbation_pi = (float)((double)A.perturbation * M_PI);
-      A.prev_w = (float)(iter * 4 + sweep) / total_steps;
-      A.last_filter = (iter == iters - 1 && sweep == 3 && c->opt.filter) ? 1 : 0;
-      A.sel_cur = c->sel[t & 1];
-      A.sel_prev = c->sel[(t + 1) & 1];
+      const PmSweepArgs A = pm_sweep_args(c, t);
       const int fw = (sweep & 1) ? P.H0 : P.W0;
-      auto mark = [&](int idx) {
-        const size_t id = (size_t)t * 4 + idx;
-        while (c->sweep_ev.size() <= id) { cudaEvent_t e; cudaEventCreate(&e); c->sweep_ev.push_back(e); }
-        cudaEventRecord(c->sweep_ev[id], s);
+      auto event = [&](std::vector<cudaEvent_t>& evs, size_t id) {
+        while (evs.size() <= id) { cudaEvent_t e; cudaEventCreate(&e); evs.push_back(e); }
+        return evs[id];
       };
+      auto mark = [&](int idx) { cudaEventRecord(event(c->sweep_ev, (size_t)t * 4 + idx), s); };
       mark(0);
-      A.rand_hyp = c->rand_hyp; A.ntrials = c->ntrials; A.usamp = c->usamp; A.prior3 = c->prior3; A.tab3 = c->tab3; A.gtab2 = c->gtab2;
-      A.fwd_pred = c->fwd_pred;
-      A.prune = (c->prune == 1) ? ((t >= c->prune_from) ? 1 : 0) : c->prune;
-      // pass M (messages) runs beside pass R (random hypotheses): both only read the state the last sweep left
-      cudaEventRecord(c->fork_ev, s);
-      cudaStreamWaitEvent(c->stream2, c->fork_ev, 0);
-      pm_msg_kernel<<<(fw * P.N + 127) / 128, 128, 0, c->stream2>>>(P, A);
-      cudaEventRecord(c->join_ev, c->stream2);
-      pm_rand_kernel<<<(fw + 63) / 64, 64, 0, s>>>(P, A);
-      cudaStreamWaitEvent(s, c->join_ev, 0);
+      event(c->rm_ev, (size_t)t * 3 + 2);   // creates the sweep's three R and M events
+      pm_launch_rand_msg(c, A, &c->rm_ev[(size_t)t * 3]);
       mark(1);
       const size_t npx = (size_t)fw * ((sweep & 1) ? P.W0 : P.H0);
       const int pgrid = (int)((npx + 4 * PM_PIXELS_PER_WARP - 1) / (4 * PM_PIXELS_PER_WARP));
@@ -1856,16 +1973,22 @@ int b200pm_run(b200pm_handle c) {
   PM_CUDA(cudaGetLastError());
   PM_CUDA(cudaEventElapsedTime(&c->last_ms, c->ev[0], c->ev[2]));
   PM_CUDA(cudaEventElapsedTime(&c->last_sweep_ms, c->ev[1], c->ev[2]));
-  c->last_kernel_ms[0] = c->last_kernel_ms[1] = c->last_kernel_ms[2] = 0.0f;
-  c->last_sweep_pass_ms.assign((size_t)t * 3, 0.0f);
-  for (int i = 0; i < t; ++i)
-    for (int kk = 0; kk < 3; ++kk) {
+  c->last_sweeps = t;
+  for (float& ms : c->last_kernel_ms) ms = 0.0f;
+  c->last_sweep_pass_ms.assign((size_t)t * PM_NUM_PASS_TIMES, 0.0f);
+  for (int i = 0; i < t; ++i) {
+    const cudaEvent_t* sw = &c->sweep_ev[(size_t)i * 4];
+    const cudaEvent_t* rm = &c->rm_ev[(size_t)i * 3];
+    const cudaEvent_t from[PM_NUM_PASS_TIMES] = {sw[0], sw[1], sw[2], sw[0], rm[1]};
+    const cudaEvent_t to[PM_NUM_PASS_TIMES] = {sw[1], sw[2], sw[3], rm[0], rm[2]};
+    for (int kk = 0; kk < PM_NUM_PASS_TIMES; ++kk) {
       float ms = 0.0f;
-      if (cudaEventElapsedTime(&ms, c->sweep_ev[(size_t)i * 4 + kk], c->sweep_ev[(size_t)i * 4 + kk + 1]) == cudaSuccess) {
+      if (cudaEventElapsedTime(&ms, from[kk], to[kk]) == cudaSuccess) {
         c->last_kernel_ms[kk] += ms;
-        c->last_sweep_pass_ms[(size_t)i * 3 + kk] = ms;
+        c->last_sweep_pass_ms[(size_t)i * PM_NUM_PASS_TIMES + kk] = ms;
       }
     }
+  }
   c->last_launches = launches;
   c->ran = true;
   return 0;
@@ -1874,10 +1997,14 @@ int b200pm_run(b200pm_handle c) {
 float b200pm_last_run_ms(b200pm_handle c) { return c ? c->last_ms : -1.0f; }
 float b200pm_last_sweep_ms(b200pm_handle c) { return c ? c->last_sweep_ms : -1.0f; }
 int b200pm_last_num_launches(b200pm_handle c) { return c ? c->last_launches : -1; }
-float b200pm_last_pass_ms(b200pm_handle c, int which) { return (c && which >= 0 && which < 3) ? c->last_kernel_ms[which] : -1.0f; }
+float b200pm_last_pass_ms(b200pm_handle c, int which) {
+  return (c && which >= 0 && which < PM_NUM_PASS_TIMES) ? c->last_kernel_ms[which] : -1.0f;
+}
 float b200pm_last_sweep_pass_ms(b200pm_handle c, int sweep, int which) {
-  if (!c || which < 0 || which >= 3 || sweep < 0 || (size_t)sweep * 3 >= c->last_sweep_pass_ms.size()) return -1.0f;
-  return c->last_sweep_pass_ms[(size_t)sweep * 3 + which];
+  if (!c || which < 0 || which >= PM_NUM_PASS_TIMES || sweep < 0 ||
+      (size_t)sweep * PM_NUM_PASS_TIMES >= c->last_sweep_pass_ms.size())
+    return -1.0f;
+  return c->last_sweep_pass_ms[(size_t)sweep * PM_NUM_PASS_TIMES + which];
 }
 size_t b200pm_patch_store_bytes(b200pm_handle c) { return c ? c->patch_store_bytes : 0; }
 
@@ -1961,6 +2088,7 @@ void b200pm_destroy(b200pm_handle c) {
   for (auto& a : c->allocs) B200DeviceCache::get().free(a.first, a.second);
   for (int i = 0; i < 4; ++i) if (c->ev[i]) cudaEventDestroy(c->ev[i]);
   for (cudaEvent_t e : c->sweep_ev) cudaEventDestroy(e);
+  for (cudaEvent_t e : c->rm_ev) cudaEventDestroy(e);
   if (c->fork_ev) cudaEventDestroy(c->fork_ev);
   if (c->join_ev) cudaEventDestroy(c->join_ev);
   if (c->stream2) { cudaStreamSynchronize(c->stream2); cudaStreamDestroy(c->stream2); }
@@ -1987,6 +2115,98 @@ int b200pm_debug_get_tab3(b200pm_handle c, float* out) {
   PM_CUDA(cudaSetDevice(c->device));
   const size_t n = (size_t)c->P.W0 * c->P.H0;
   PM_CUDA(cudaMemcpy(out, c->tab3, sizeof(float) * 3 * n * c->P.N, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+// debug: passes R and M of the sweep that follows the last run (sweep t = the run's sweep count, which B200PM_MAX_SWEEPS
+// sets), on the state that run left.  Out, pixels in the original orientation: rand_hyp [pixel][4], usamp
+// [pixel][num_samples], the backward messages sel [pixel][N] (pass S overwrites them with the selection probabilities,
+// so they are read here, before any pass S), fwd [pixel][N], and the RNG border slots [2 W + 2 H][6] after pass R.  The
+// handle's maps are unchanged; its RNG slots advance as that sweep's pass R advances them.
+int b200pm_debug_rand_msg(b200pm_handle c, float* rand_hyp, float* usamp, float* sel, float* fwd, uint32_t* rng) {
+  if (!c) return pm_fail(-1, "null handle");
+  if (!c->ran || c->last_sweeps >= 4 * c->opt.num_iterations) return pm_fail(-1, "no sweep follows the last run");
+  PM_CUDA(cudaSetDevice(c->device));
+  const PmParams& P = c->P;
+  const size_t n = (size_t)P.W0 * P.H0, nN = n * P.N;
+  const PmSweepArgs A = pm_sweep_args(c, c->last_sweeps);
+  pm_launch_rand_msg(c, A, nullptr);
+  PM_CUDA(cudaStreamSynchronize(c->stream));
+  PM_CUDA(cudaGetLastError());
+  PM_CUDA(cudaMemcpy(rand_hyp, A.rand_hyp, sizeof(float4) * n, cudaMemcpyDeviceToHost));
+  PM_CUDA(cudaMemcpy(usamp, A.usamp, sizeof(float) * n * P.num_samples, cudaMemcpyDeviceToHost));
+  PM_CUDA(cudaMemcpy(sel, A.sel_cur, sizeof(float) * nN, cudaMemcpyDeviceToHost));
+  PM_CUDA(cudaMemcpy(fwd, A.fwd_pred, sizeof(float) * nN, cudaMemcpyDeviceToHost));
+  PM_CUDA(cudaMemcpy(rng, P.rng, sizeof(uint32_t) * 6 * (2 * (size_t)P.W0 + 2 * (size_t)P.H0), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+// The column-serial statement of pass R: one column's rows in order, each from where the previous one left the stream.
+static void pm_rand_column_host(const PmParams& P, const PmSweepArgs& A, const float4* hyp, uint32_t* rng, int col,
+                                float4* rand_hyp, float* usamp, uint8_t* rounds) {
+  const int rot = A.rot;
+  const int fh = (rot & 1) ? P.W0 : P.H0;
+  const float iK[4] = {P.invK[rot][0], P.invK[rot][1], P.invK[rot][2], P.invK[rot][3]};
+  int r0, c0;
+  pm_frame_to_orig(P.W0, P.H0, rot, 0, col, &r0, &c0);
+  uint32_t* slot = rng + 6 * (size_t)pm_border_index(P.W0, P.H0, r0, c0);
+  PmRng rs;
+  rs.v0 = slot[0]; rs.v1 = slot[1]; rs.v2 = slot[2]; rs.v3 = slot[3]; rs.v4 = slot[4]; rs.d = slot[5];
+  const float colf = (float)col;
+  for (int row = 0; row < fh; ++row) {
+    const size_t p = pm_pix0(P.W0, P.H0, rot, row, col);
+    const float4 cur4 = hyp[p];
+    float n0 = cur4.y, n1 = cur4.z;
+    pm_normal_to_frame(rot, n0, n1);
+    const float dmin = (1.0f - A.perturbation) * cur4.x;
+    const float dmax = (1.0f + A.perturbation) * cur4.x;
+    const float rand_d = fmaf(pm_rng_uniform(rs), dmax - dmin, dmin);
+    float rn[3];
+    rounds[p] = (uint8_t)pm_perturb_normal(iK, (float)row, colf, A.perturbation_pi, n0, n1, cur4.w, rs, rn);
+    rand_hyp[p] = make_float4(rand_d, rn[0], rn[1], rn[2]);
+    for (int s = 0; s < P.num_samples; ++s) usamp[p * P.num_samples + s] = pm_rng_uniform(rs) - FLT_EPSILON;
+  }
+  slot[0] = rs.v0; slot[1] = rs.v1; slot[2] = rs.v2; slot[3] = rs.v3; slot[4] = rs.v4; slot[5] = rs.d;
+}
+// The column-serial statement of pass M for one (column, image): the backward recurrence, then the forward one.
+static void pm_msg_column_host(const PmParams& P, const PmSweepArgs& A, const float* cost, int col, int img, float* sel,
+                               float* fwd) {
+  const int rot = A.rot, N = P.N;
+  const int fh = (rot & 1) ? P.W0 : P.H0;
+  float beta = 0.5f;
+  for (int row = fh - 1; row >= 0; --row) {
+    const size_t p = pm_pix0(P.W0, P.H0, rot, row, col);
+    beta = pm_backward_message(P.L, cost[p * N + img], beta);
+    sel[p * N + img] = beta;
+  }
+  float f = 0.5f;
+  for (int row = 0; row < fh; ++row) {
+    const size_t p = pm_pix0(P.W0, P.H0, rot, row, col);
+    f = pm_forward_message(P.L, cost[p * N + img], f);
+    fwd[p * N + img] = f;
+  }
+}
+
+// test: what b200pm_debug_rand_msg returns, computed on the host by pm_rand_column_host and pm_msg_column_host from the
+// device state the last run left, plus the PerturbNormal rounds of every pixel (rounds [pixel]).  Changes nothing.
+int b200pm_test_rand_msg(b200pm_handle c, float* rand_hyp, float* usamp, float* sel, float* fwd, uint32_t* rng,
+                         uint8_t* rounds) {
+  if (!c) return pm_fail(-1, "null handle");
+  if (!c->ran || c->last_sweeps >= 4 * c->opt.num_iterations) return pm_fail(-1, "no sweep follows the last run");
+  PM_CUDA(cudaSetDevice(c->device));
+  const PmParams& P = c->P;
+  const size_t n = (size_t)P.W0 * P.H0;
+  const PmSweepArgs A = pm_sweep_args(c, c->last_sweeps);
+  std::vector<float4> hyp(n);
+  std::vector<float> cost(n * P.N);
+  PM_CUDA(cudaMemcpy(hyp.data(), P.hyp, sizeof(float4) * n, cudaMemcpyDeviceToHost));
+  PM_CUDA(cudaMemcpy(cost.data(), P.cost, sizeof(float) * n * P.N, cudaMemcpyDeviceToHost));
+  PM_CUDA(cudaMemcpy(rng, P.rng, sizeof(uint32_t) * 6 * (2 * (size_t)P.W0 + 2 * (size_t)P.H0), cudaMemcpyDeviceToHost));
+  const int fw = (A.rot & 1) ? P.H0 : P.W0;
+  for (int col = 0; col < fw; ++col) {
+    pm_rand_column_host(P, A, hyp.data(), rng, col, reinterpret_cast<float4*>(rand_hyp), usamp, rounds);
+    for (int img = 0; img < P.N; ++img) pm_msg_column_host(P, A, cost.data(), col, img, sel, fwd);
+  }
   return 0;
 }
 

@@ -295,7 +295,8 @@ class PatchMatch:
         return float(self._lib.b200pm_last_pass_ms(self._h, which))
 
     def last_sweep_pass_ms(self, sweep, which):
-        """Device time of one pass (0 = rand + msg, 1 = pixel, 2 = serial) in one sweep of the last run."""
+        """Device time of one pass (0 = rand + msg side by side, 1 = pixel, 2 = serial, 3 = rand alone, 4 = msg alone)
+        in one sweep of the last run."""
         return float(self._lib.b200pm_last_sweep_pass_ms(self._h, sweep, which))
 
     def patch_store_bytes(self):

@@ -103,8 +103,10 @@ float b200pm_last_run_ms(b200pm_handle h);
 /* Device time spent in the sweep kernels only during the last run, and their launch count. */
 float b200pm_last_sweep_ms(b200pm_handle h);
 int b200pm_last_num_launches(b200pm_handle h);
-/* Device time summed over the sweeps of the last run for one pass of the split sweep: 0 = pm_rand_kernel (column-serial
- * PRNG pass), 1 = pm_pixel_kernel (pixel-parallel NCC pass, the dominant kernel), 2 = pm_serial_kernel. */
+/* Device time summed over the sweeps of the last run for one pass of the split sweep: 0 = pm_rand_kernel and
+ * pm_msg_kernel, which run side by side (from the sweep's start until both are done), 1 = pm_pixel_kernel
+ * (pixel-parallel NCC pass, the dominant kernel), 2 = pm_serial_kernel, 3 = pm_rand_kernel alone, 4 = pm_msg_kernel
+ * alone (its own stream).  0, 1 and 2 add up to the sweep; 3 and 4 overlap inside 0. */
 float b200pm_last_pass_ms(b200pm_handle h, int which);
 /* The same for one sweep of the last run (sweep t runs in frame t % 4; -1 for a sweep that did not run). */
 float b200pm_last_sweep_pass_ms(b200pm_handle h, int sweep, int which);
