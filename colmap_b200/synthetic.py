@@ -700,3 +700,57 @@ def synthesize_pose_graph(rec, noise_deg=0.0, outlier_ratio=0.0, seed=0, gravity
             pg.AddEdge(i1, i2, PoseGraphEdge(np.concatenate([_R_to_quat(R12), np.zeros(3)]), n))
     priors = [PosePrior(i, gravity=R[i] @ np.array([0.0, 1.0, 0.0])) for i in ids] if gravity else []
     return pg, priors
+
+
+# --------------------------------------------------------------------------------------------------
+# SIFT descriptors
+# --------------------------------------------------------------------------------------------------
+def FeatureDescriptorsToUnsignedByte(x):
+    """FeatureDescriptorsToUnsignedByte (feature/utils.cc:57-69): round(512 x) (half away from zero), clamped to
+    [0, 255], in float32."""
+    s = np.float32(512.0) * np.asarray(x, np.float32)
+    r = np.sign(s) * np.floor(np.abs(s) + np.float32(0.5))
+    return np.clip(r, 0, 255).astype(np.uint8)
+
+
+def CreateRandomFeatureDescriptors(num_features, seed=0):
+    """The descriptors of the reference's matcher tests (feature/sift_test.cc:211-227): 10 random dimensions set to 1,
+    L2-normalised, to uint8.  Every row is 162 on 10 dimensions and 0 elsewhere, so dot products between rows take
+    few distinct values and tie often."""
+    rng = np.random.default_rng(seed)
+    x = np.zeros((num_features, 128), np.float32)
+    if num_features:
+        dims = np.argsort(rng.random((num_features, 128)), axis=1)[:, :10]
+        np.put_along_axis(x, dims, np.float32(1.0), axis=1)
+        x /= np.linalg.norm(x, axis=1, keepdims=True).astype(np.float32)
+    return FeatureDescriptorsToUnsignedByte(x)
+
+
+def _sift_like(rng, n):
+    """Non-negative, sparse-ish unit rows, clipped at 0.2 and renormalised as SIFT does, in float32."""
+    x = rng.gamma(0.6, 1.0, (n, 128)).astype(np.float32)
+    x /= np.linalg.norm(x, axis=1, keepdims=True)
+    x = np.minimum(x, np.float32(0.2))
+    return x / np.linalg.norm(x, axis=1, keepdims=True)
+
+
+def make_sift_view_pair(n1, n2, overlap=0.5, noise=(0.0, 3.0), seed=0):
+    """Descriptors of two overlapping views, (n1, 128) and (n2, 128) uint8.  Image 2 holds noisy copies of a random
+    subset of image 1's rows (min(n1, n2) * overlap of them, each with its own noise level drawn from `noise`, relative
+    to the row's norm), the rest are unrelated distractors, in a random order.  The spread of noise levels puts many
+    rows on both sides of the ratio and distance thresholds.  Returns (desc1, desc2, truth), truth[k] = (i1, i2) of
+    each planted copy."""
+    rng = np.random.default_rng(seed)
+    a = _sift_like(rng, n1)
+    k = int(min(n1, n2) * overlap)
+    src = rng.choice(n1, size=k, replace=False) if k else np.zeros(0, np.int64)
+    sigma = rng.uniform(noise[0], noise[1], (k, 1)).astype(np.float32)
+    copies = a[src] + sigma * np.abs(rng.normal(0, 1, (k, 128))).astype(np.float32) / np.sqrt(np.float32(128))
+    copies = np.maximum(copies, 0)
+    copies /= np.maximum(np.linalg.norm(copies, axis=1, keepdims=True), np.float32(1e-12))
+    b = np.concatenate([copies, _sift_like(rng, n2 - k)], axis=0)
+    perm = rng.permutation(n2)
+    b = b[perm]
+    inv = np.empty(n2, np.int64); inv[perm] = np.arange(n2)
+    truth = np.stack([src, inv[np.arange(k)]], axis=1) if k else np.zeros((0, 2), np.int64)
+    return FeatureDescriptorsToUnsignedByte(a), FeatureDescriptorsToUnsignedByte(b), truth
