@@ -1073,6 +1073,34 @@ __global__ void ba_invert_blocks_kernel(const BaDev D) {
 // ------------------------------------------------------------------------------------------------
 // PCG on the reduced camera system; all scalars live in D.ctl, kernels are no-ops once ctl->done is set.
 // ------------------------------------------------------------------------------------------------
+// z_i = (M^-1)_i . r over the block of row i (ri = D.row_info[i], rblock = r + ri.x).  The row of M^-1 is fetched with
+// one batch of predicated loads instead of a dependent load per column; the columns past 11 of a wide block follow.
+__device__ __forceinline__ double ba_precond_row(int4 ri, const double* __restrict__ Minv, const double* rblock) {
+  const double* __restrict__ M = Minv + ri.y;
+  double m[11];
+#pragma unroll
+  for (int k = 0; k < 11; ++k) m[k] = k < ri.z ? M[k] : 0.0;
+  double t = 0;
+#pragma unroll
+  for (int k = 0; k < 11; ++k) if (k < ri.z) t += m[k] * rblock[k];
+  for (int k = 11; k < ri.z; ++k) t += M[k] * rblock[k];
+  return t;
+}
+// The end of a PCG iteration, after `it` completed ones: scalar bookkeeping and termination, in one thread.  Returns
+// done.  Inexact mode: ceres ConjugateGradientsSolver's Q-tolerance, zeta = it (Q1 - Q0) / Q1 below eta.  Exact mode
+// (DENSE_/SPARSE_SCHUR requested): relative residual |r| <= r_tolerance |b|.
+__device__ __forceinline__ int ba_pcg_end_iteration(BaCtl* c, int it, double rho, double Q0, double Q1, double rnorm2,
+                                                    double norm_b, double q_tolerance, double r_tolerance, int max_iters) {
+  it += 1;
+  const bool converged = r_tolerance > 0.0 ? rnorm2 <= r_tolerance * r_tolerance * norm_b : it * (Q1 - Q0) / Q1 < q_tolerance;
+  const int done = converged || it >= max_iters;
+  c->it = it; c->iters_total += 1;
+  c->Q0 = Q1; c->Q1 = 0.0; c->rnorm2 = 0.0;
+  c->last_rho = rho; c->rho = 0.0; c->pq = 0.0;
+  c->done = done;
+  return done;
+}
+
 __global__ void ba_pcg_init_kernel(const BaDev D) {  // x = 0, r = b, norm_b
   __shared__ double sm[8];
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1088,10 +1116,8 @@ __global__ void ba_pcg_precond_kernel(const BaDev D) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   double v = 0;
   if (i < D.nc) {
-    const int b = D.off2blk[i], n = D.blk_start[b + 1] - D.blk_start[b], l = i - D.blk_start[b];
-    const double* M = D.Minv + D.blk_pack[b] + l * n;
-    double t = 0;
-    for (int c = 0; c < n; ++c) t += M[c] * D.rr[D.blk_start[b] + c];
+    const int4 ri = D.row_info[i];
+    const double t = ba_precond_row(ri, D.Minv, D.rr + ri.x);
     D.z[i] = t;
     v = t * D.rr[i];
   }
@@ -1363,15 +1389,25 @@ __device__ __forceinline__ double ba_cta_allsum(double v, double* sm /* [33] */)
   __syncthreads();
   return t;  // valid in every thread
 }
+// Two sums in one pass through the barriers, for a CTA of BA_PCG_T threads (32 warps); the totals are valid in thread 0.
+__device__ __forceinline__ void ba_cta_sum2(double& a, double& w, double (*sm2)[33]) {
+  for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); w += __shfl_xor_sync(0xffffffffu, w, o); }
+  const int wid = threadIdx.x >> 5, l = threadIdx.x & 31;
+  if (l == 0) { sm2[0][wid] = a; sm2[1][wid] = w; }
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    a = sm2[0][threadIdx.x]; w = sm2[1][threadIdx.x];
+    for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); w += __shfl_xor_sync(0xffffffffu, w, o); }
+  }
+}
 // One launch between two SpMVs: the tail of PCG iteration i (pq = p.q ; x += alpha p ; r -= alpha q ; Q1 = -x.(b + r) ;
-// |r|^2 ; termination, see ba_pcg_step_kernel) followed by the head of iteration i + 1 (z = M^-1 r ; rho = r.z ;
+// |r|^2 ; termination, see ba_pcg_end_iteration) followed by the head of iteration i + 1 (z = M^-1 r ; rho = r.z ;
 // p = z + beta p ; q = D_c^2 p — the SpMV adds the rest).  do_post = 0 for the very first call of a solve.
-#define BA_PCG_EPT 4   // elements per thread handled from registers (nc <= BA_PCG_T * BA_PCG_EPT takes the fast path;
-                      // tests/test_ba_paths_gpu.py mirrors this threshold)
 __global__ void __launch_bounds__(BA_PCG_T) ba_pcg_mid_kernel(const BaDev D, double q_tolerance, double r_tolerance,
                                                               int max_iters, int zero_q, int do_post, int r_in_smem) {
   extern __shared__ double s_r[];   // [nc] when r_in_smem
   __shared__ double sm[33];
+  __shared__ double sm2[2][33];
   __shared__ int s_done;
   BaCtl* c = D.ctl;
   if (c->done) return;
@@ -1384,71 +1420,29 @@ __global__ void __launch_bounds__(BA_PCG_T) ba_pcg_mid_kernel(const BaDev D, dou
   double last_rho = c->last_rho;
   const double rho_in = c->rho, norm_b = c->norm_b, Q0 = c->Q0;
   if (do_post) {
-    double pv[BA_PCG_EPT], qv[BA_PCG_EPT], v = 0.0;
-    const bool small = nc <= BA_PCG_T * BA_PCG_EPT;
-    if (small) {
-#pragma unroll
-      for (int e = 0; e < BA_PCG_EPT; ++e) { const int i = threadIdx.x + e * BA_PCG_T; pv[e] = i < nc ? P[i] : 0.0; qv[e] = i < nc ? Q[i] : 0.0; v += pv[e] * qv[e]; }
-    } else {
-      for (int i = threadIdx.x; i < nc; i += BA_PCG_T) v += P[i] * Q[i];
-    }
+    double v = 0.0;
+    for (int i = threadIdx.x; i < nc; i += BA_PCG_T) v += P[i] * Q[i];
     const double pq = ba_cta_allsum(v, sm);
     if (!(pq > 0.0)) { if (threadIdx.x == 0) c->done = 1; return; }
     const double alpha = rho_in / pq;
     double a = 0.0, w = 0.0;
-    if (small) {
-      double xv[BA_PCG_EPT], rv[BA_PCG_EPT], bv[BA_PCG_EPT];
-#pragma unroll
-      for (int e = 0; e < BA_PCG_EPT; ++e) { const int i = threadIdx.x + e * BA_PCG_T; xv[e] = i < nc ? X[i] : 0.0; rv[e] = i < nc ? R[i] : 0.0; bv[e] = i < nc ? RHS[i] : 0.0; }
-#pragma unroll
-      for (int e = 0; e < BA_PCG_EPT; ++e) {
-        const int i = threadIdx.x + e * BA_PCG_T;
-        const double x = xv[e] + alpha * pv[e], r = rv[e] - alpha * qv[e];
-        if (i < nc) { X[i] = x; R[i] = r; if (r_in_smem) s_r[i] = r; a += -x * (bv[e] + r); w += r * r; }
-      }
-    } else {
-      for (int i = threadIdx.x; i < nc; i += BA_PCG_T) {
-        const double x = X[i] + alpha * P[i];
-        const double r = R[i] - alpha * Q[i];
-        X[i] = x; R[i] = r;
-        if (r_in_smem) s_r[i] = r;
-        a += -x * (RHS[i] + r);
-        w += r * r;
-      }
+    for (int i = threadIdx.x; i < nc; i += BA_PCG_T) {
+      const double x = X[i] + alpha * P[i];
+      const double r = R[i] - alpha * Q[i];
+      X[i] = x; R[i] = r;
+      if (r_in_smem) s_r[i] = r;
+      a += -x * (RHS[i] + r);
+      w += r * r;
     }
-    // two sums in one pass through the barriers
-    for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); w += __shfl_xor_sync(0xffffffffu, w, o); }
-    __shared__ double sm2[2][33];
-    const int wid = threadIdx.x >> 5, l = threadIdx.x & 31;
-    if (l == 0) { sm2[0][wid] = a; sm2[1][wid] = w; }
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      double ta = sm2[0][threadIdx.x], tw = sm2[1][threadIdx.x];   // BA_PCG_T / 32 == 32 warps
-      for (int o = 16; o > 0; o >>= 1) { ta += __shfl_xor_sync(0xffffffffu, ta, o); tw += __shfl_xor_sync(0xffffffffu, tw, o); }
-      if (threadIdx.x == 0) {
-        const double Q1 = ta, rnorm2 = tw;
-        int done = 0;
-        c->it = it + 1; c->iters_total += 1;
-        if (r_tolerance > 0.0) {
-          if (rnorm2 <= r_tolerance * r_tolerance * norm_b || it + 1 >= max_iters) done = 1;
-        } else {
-          const double zeta = (it + 1) * (Q1 - Q0) / Q1;
-          if (zeta < q_tolerance || it + 1 >= max_iters) done = 1;
-        }
-        c->Q0 = Q1; c->Q1 = 0.0; c->rnorm2 = 0.0;
-        c->last_rho = rho_in; c->rho = 0.0; c->pq = 0.0;
-        c->done = done;
-        s_done = done;
-      }
-    }
+    ba_cta_sum2(a, w, sm2);
+    if (threadIdx.x == 0) s_done = ba_pcg_end_iteration(c, it, rho_in, Q0, a, w, norm_b, q_tolerance, r_tolerance, max_iters);
     __syncthreads();   // also orders the R stores above before the preconditioner reads below
     if (s_done) return;
     it += 1;
     last_rho = rho_in;
   }
   // z = M^-1 r, block row by block row.  The residual of the whole camera side sits in shared memory when it fits (the
-  // rows of a block belong to different threads), and the row of M^-1 is fetched with one batch of predicated loads
-  // instead of a dependent load per column: this kernel is a chain of latencies, not of bytes.
+  // rows of a block belong to different threads): this kernel is a chain of latencies, not of bytes.
   if (r_in_smem && !do_post) {
     for (int i = threadIdx.x; i < nc; i += BA_PCG_T) s_r[i] = R[i];
     __syncthreads();
@@ -1456,16 +1450,8 @@ __global__ void __launch_bounds__(BA_PCG_T) ba_pcg_mid_kernel(const BaDev D, dou
   const double* __restrict__ RV = r_in_smem ? s_r : R;
   double v = 0.0;
   for (int i = threadIdx.x; i < nc; i += BA_PCG_T) {
-    const int4 ri = D.row_info[i];   // {first row of the block, offset of this row of Minv, block size}
-    const double* __restrict__ M = MI + ri.y;
-    const double* __restrict__ rb = RV + ri.x;
-    double m[11];
-#pragma unroll
-    for (int k = 0; k < 11; ++k) m[k] = k < ri.z ? M[k] : 0.0;
-    double t = 0;
-#pragma unroll
-    for (int k = 0; k < 11; ++k) if (k < ri.z) t += m[k] * rb[k];
-    for (int k = 11; k < ri.z; ++k) t += M[k] * rb[k];
+    const int4 ri = D.row_info[i];
+    const double t = ba_precond_row(ri, MI, RV + ri.x);
     Z[i] = t;
     v += t * RV[i];
   }
@@ -1542,29 +1528,8 @@ __global__ void __launch_bounds__(BA_PCG_T) ba_pcg_mid_staged_kernel(const BaDev
         a += -x * (s_b[i] + r); w += r * r;
       }
     }
-    for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); w += __shfl_xor_sync(0xffffffffu, w, o); }
-    const int wid = threadIdx.x >> 5, l = threadIdx.x & 31;
-    if (l == 0) { sm2[0][wid] = a; sm2[1][wid] = w; }
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      double ta = sm2[0][threadIdx.x], tw = sm2[1][threadIdx.x];   // BA_PCG_T / 32 == 32 warps
-      for (int o = 16; o > 0; o >>= 1) { ta += __shfl_xor_sync(0xffffffffu, ta, o); tw += __shfl_xor_sync(0xffffffffu, tw, o); }
-      if (threadIdx.x == 0) {
-        const double Q1 = ta, rnorm2 = tw;
-        int done = 0;
-        c->it = it + 1; c->iters_total += 1;
-        if (r_tolerance > 0.0) {
-          if (rnorm2 <= r_tolerance * r_tolerance * norm_b || it + 1 >= max_iters) done = 1;
-        } else {
-          const double zeta = (it + 1) * (Q1 - Q0) / Q1;
-          if (zeta < q_tolerance || it + 1 >= max_iters) done = 1;
-        }
-        c->Q0 = Q1; c->Q1 = 0.0; c->rnorm2 = 0.0;
-        c->last_rho = rho_in; c->rho = 0.0; c->pq = 0.0;
-        c->done = done;
-        s_done = done;
-      }
-    }
+    ba_cta_sum2(a, w, sm2);
+    if (threadIdx.x == 0) s_done = ba_pcg_end_iteration(c, it, rho_in, Q0, a, w, norm_b, q_tolerance, r_tolerance, max_iters);
     __syncthreads();   // publishes s_r (the rows of a block belong to different threads)
     if (s_done) return;
     it += 1;
@@ -1581,16 +1546,8 @@ __global__ void __launch_bounds__(BA_PCG_T) ba_pcg_mid_staged_kernel(const BaDev
     const int i = threadIdx.x + e * BA_PCG_T;
     zv[e] = 0.0;
     if (i < nc) {
-      const int4 ri = s_ri[i];   // {first row of the block, offset of this row of Minv, block size}
-      const double* __restrict__ M = MI + ri.y;
-      const double* rb = s_r + ri.x;
-      double m[11];
-#pragma unroll
-      for (int k = 0; k < 11; ++k) m[k] = k < ri.z ? M[k] : 0.0;
-      double t = 0;
-#pragma unroll
-      for (int k = 0; k < 11; ++k) if (k < ri.z) t += m[k] * rb[k];
-      for (int k = 11; k < ri.z; ++k) t += M[k] * rb[k];
+      const int4 ri = s_ri[i];
+      const double t = ba_precond_row(ri, MI, s_r + ri.x);
       Z[i] = t; zv[e] = t;
       v += t * s_r[i];
     }
@@ -1637,21 +1594,11 @@ __global__ void ba_pcg_update_kernel(const BaDev D) {
   const double t2 = ba_block_sum(w, sm);
   if (threadIdx.x == 0) { atomicAdd(&D.ctl->Q1, t); atomicAdd(&D.ctl->rnorm2, t2); }
 }
-// scalar bookkeeping + termination.  Inexact mode: ceres ConjugateGradientsSolver's Q-tolerance (zeta < eta).
-// Exact mode (DENSE_/SPARSE_SCHUR requested): relative residual |r| <= r_tolerance |b|.
 __global__ void ba_pcg_step_kernel(const BaDev D, double q_tolerance, double r_tolerance, int max_iters) {
   BaCtl* c = D.ctl;
   if (c->done) return;
   if (!(c->pq > 0.0)) { c->done = 1; return; }
-  c->it += 1; c->iters_total += 1;
-  if (r_tolerance > 0.0) {
-    if (c->rnorm2 <= r_tolerance * r_tolerance * c->norm_b || c->it >= max_iters) c->done = 1;
-  } else {
-    const double zeta = c->it * (c->Q1 - c->Q0) / c->Q1;
-    if (zeta < q_tolerance || c->it >= max_iters) c->done = 1;
-  }
-  c->Q0 = c->Q1; c->Q1 = 0.0; c->rnorm2 = 0.0;
-  c->last_rho = c->rho; c->rho = 0.0; c->pq = 0.0;
+  ba_pcg_end_iteration(c, c->it, c->rho, c->Q0, c->Q1, c->rnorm2, c->norm_b, q_tolerance, r_tolerance, max_iters);
 }
 
 // Generic path for tracks longer than a block (> 256 observations; rare): the per-point sum goes through global
@@ -2077,7 +2024,8 @@ struct BaPool {
 
 static int ba_sm_count() { int dev = 0, n = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); return n; }
 // The reduced-system kernels of one solve, chosen once per solve by ba_select_path from nc and the solver type.
-// B200BA_NO_DENSE, B200BA_PCG_MULTI, B200BA_MID_GLOBAL, B200BA_MID_PLAIN and B200BA_SPMV_SMEM=0 turn a path off (test seams).
+// B200BA_NO_DENSE, B200BA_PCG_MULTI, B200BA_MID_GLOBAL, B200BA_MID_PLAIN and B200BA_SPMV_SMEM=0 turn a path off (test
+// seams).  B200BA_MID_PLAIN runs small problems through ba_pcg_mid_kernel, the loop that larger ones (B5) take.
 struct BaPath {
   bool dense;          // dense Cholesky of the explicit reduced camera matrix
   bool fused_pcg;      // single-CTA PCG vector step between the SpMVs (else five kernels per iteration)

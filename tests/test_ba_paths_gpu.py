@@ -36,7 +36,6 @@ from test_ba_gpu import _assert_parity, _both, _gauge
 DENSE_MAX = 256                  # BA_DENSE_MAX: exact requests up to this nc factorise the reduced matrix densely
 PCG_FUSED_MAX = 65536            # BA_PCG_FUSED_MAX: single-CTA PCG vector step between SpMVs; above: five kernels
 MID_STAGED_MAX = 1024 * 5        # BA_PCG_T * BA_MID_EPT: ba_pcg_mid_staged_kernel
-MID_SMALL_MAX = 1024 * 4         # BA_PCG_T * BA_PCG_EPT: the register (`small`) branch of ba_pcg_mid_kernel
 MID_SMEM_MAX = 160 * 1024 // 8   # the 160 KB dynamic shared memory of ba_pcg_mid_kernel: r in shared memory
 SPMV_SMEM_MAX = 72 * 1024 // 8   # BA_SPMV_SMEM_MAX: SpMV pass 1 with p in shared memory
 NARROW_MODELS = (0, 1, 2, 3, 8, 9)   # ba_model_is_narrow: hand-written Jacobians, DC = 6 + dkmax
@@ -56,7 +55,7 @@ def regime(flat, options, env=None):
         nimg = flat.num_config_images or len(np.unique(flat.obs_pose))
         lst = DENSE_SCHUR if nimg <= 50 else (SPARSE_SCHUR if nimg <= 1000 else ITERATIVE_SCHUR)
     exact = lst != ITERATIVE_SCHUR
-    r = dict(nc=nc, dkmax=dkmax, DC=DC, lst=lst, exact=exact, mid_small=False, spmv=None)
+    r = dict(nc=nc, dkmax=dkmax, DC=DC, lst=lst, exact=exact, spmv=None)
     if exact and nc <= DENSE_MAX and "B200BA_NO_DENSE" not in env:
         r["path"] = "dense"
         return r
@@ -67,7 +66,6 @@ def regime(flat, options, env=None):
         r["path"] = "staged"
     else:
         r["path"] = "mid_smem" if nc <= MID_SMEM_MAX and "B200BA_MID_GLOBAL" not in env else "mid_global"
-        r["mid_small"] = nc <= MID_SMALL_MAX
     if L["nblocks_warp"] == 0:      # no track of <= 32 observations: pass 1 runs ba_schur_spmv_kernel only
         r["spmv"] = "block"
     else:
@@ -170,8 +168,8 @@ def _c(problem, options, env=(), cam_rel=1e-5, **expect):
 
 NATURAL = [
     _c("staged_ept5", ITER, path="staged", spmv="smem", nc=4794),
-    _c("mid_smem_spmv_smem", ITER, path="mid_smem", mid_small=False, spmv="smem", nc=7994),
-    _c("b5_shape", ITER, path="mid_smem", mid_small=False, spmv="global", nc=15994),
+    _c("mid_smem_spmv_smem", ITER, path="mid_smem", spmv="smem", nc=7994),
+    _c("b5_shape", ITER, path="mid_smem", spmv="global", nc=15994),
     _c("mid_global", ITER, path="mid_global", spmv="global", nc=20794),
     _c("multi", ITER, path="multi", spmv="global", nc=74694),
 ]
@@ -179,7 +177,7 @@ BOUNDARY = [
     _c("nc4096", ITER, path="staged", spmv="smem", nc=4096),
     _c("nc4097", ITER, path="staged", spmv="smem", nc=4097),
     _c("nc5120", ITER, path="staged", spmv="smem", nc=5120),
-    _c("nc5121", ITER, path="mid_smem", mid_small=False, spmv="smem", nc=5121),
+    _c("nc5121", ITER, path="mid_smem", spmv="smem", nc=5121),
     _c("nc9216", ITER, path="mid_smem", spmv="smem", nc=9216),
     _c("nc9217", ITER, path="mid_smem", spmv="global", nc=9217),
     _c("nc20480", ITER, path="mid_smem", spmv="global", nc=20480),
@@ -195,8 +193,8 @@ EXACT = [
 ]
 _SEAM_SETTINGS = [
     ((), dict(path="staged", spmv="smem")),
-    ((("B200BA_MID_PLAIN", "1"),), dict(path="mid_smem", mid_small=True, spmv="smem")),
-    ((("B200BA_MID_PLAIN", "1"), ("B200BA_MID_GLOBAL", "1")), dict(path="mid_global", mid_small=True, spmv="smem")),
+    ((("B200BA_MID_PLAIN", "1"),), dict(path="mid_smem", spmv="smem")),
+    ((("B200BA_MID_PLAIN", "1"), ("B200BA_MID_GLOBAL", "1")), dict(path="mid_global", spmv="smem")),
     ((("B200BA_PCG_MULTI", "1"),), dict(path="multi", spmv="smem")),
     ((("B200BA_SPMV_SMEM", "0"),), dict(path="staged", spmv="global")),
 ]
@@ -231,17 +229,15 @@ def test_every_case_lands_in_its_regime():
     """Host only: every case below runs the path it is named for (the thresholds above, the layout of b200ba_test_pack)."""
     rows, bad, regimes = [], [], [_regime(case) for case in ALL]
     for case, r in zip(ALL, regimes):
-        rows.append(f"{case.id:62s} nc {r['nc']:6d}  dkmax {r['dkmax']:2d}  DC {r['DC']:2d}  {r['path']:10s} "
-                    f"small {int(r['mid_small'])}  spmv {r['spmv']}")
+        rows.append(f"{case.id:62s} nc {r['nc']:6d}  dkmax {r['dkmax']:2d}  DC {r['DC']:2d}  {r['path']:10s} spmv {r['spmv']}")
         if any(r[k] != v for k, v in case.expect):
             bad.append(f"{case.id}: expected {dict(case.expect)}, got {r}")
     print("\n" + "\n".join(rows))
     assert not bad, "\n".join(bad)
     # every regime of the table is covered
-    seen = {(r["path"], r["spmv"], r["mid_small"]) for r in regimes}
-    for want in (("dense", None, False), ("staged", "smem", False), ("staged", "global", False), ("mid_smem", "smem", True),
-                 ("mid_smem", "smem", False), ("mid_smem", "global", False), ("mid_global", "global", False),
-                 ("mid_global", "smem", True), ("multi", "global", False), ("multi", "smem", False)):
+    seen = {(r["path"], r["spmv"]) for r in regimes}
+    for want in (("dense", None), ("staged", "smem"), ("staged", "global"), ("mid_smem", "smem"), ("mid_smem", "global"),
+                 ("mid_global", "global"), ("mid_global", "smem"), ("multi", "global"), ("multi", "smem")):
         assert want in seen, want
     assert max(r["dkmax"] for r in regimes) > 16
 
