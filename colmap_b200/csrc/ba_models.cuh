@@ -1,7 +1,7 @@
 // ba_models.cuh — camera models with MORE than five parameters, as formulas only, differentiated by forward-mode dual
-// numbers that live in registers (groundwork for SURVEY.md section 8f rank 4; the LM kernels of bundle_adjustment.cu
-// still take the <= 5-parameter models through their hand-written Jacobians, so nothing here is on the solve path yet —
-// it is reachable through the CPU test hook b200ba_test_project_wide only).
+// numbers that live in registers (SURVEY.md section 8f rank 4).  The solve and the covariance estimate evaluate these
+// models in every WIDE linearisation (ba_img_from_cam_any / ba_residual_any in ba_common.cuh); the <= 5-parameter
+// models keep their hand-written Jacobians.  The CPU test hook b200ba_test_project_wide evaluates them on the host.
 //
 // Reference behaviour: ImgFromCam of the twelve models COLMAP has beyond the radial pinhole family - OPENCV,
 // OPENCV_FISHEYE, FULL_OPENCV, FOV, THIN_PRISM_FISHEYE, RAD_TAN_THIN_PRISM_FISHEYE, SIMPLE_DIVISION, DIVISION,

@@ -11,8 +11,8 @@ import oracle_ba
 from colmap_b200 import load_library
 from colmap_b200.bundle_adjustment import (DENSE_SCHUR, ITERATIVE_SCHUR, PINHOLE, RADIAL, RADIAL_FISHEYE, SIMPLE_PINHOLE,
                                            SIMPLE_RADIAL_FISHEYE,
-                                           SIMPLE_RADIAL, SOFT_L1, BundleAdjustmentOptions, _CProblem, _COptions,
-                                           _bind, _f64p, _i8p, _u8p)
+                                           SIMPLE_RADIAL, SOFT_L1, BundleAdjustmentOptions, _CConfig, _CCovOptions, _CProblem,
+                                           _COptions, _CScene, _bind, _bind_cov, _f64p, _i8p, _i32p, _u8p)
 from colmap_b200.synthetic import synthesize_ba_problem
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -322,6 +322,23 @@ def test_product_rejects_unsupported_inputs_without_a_gpu():
     cp = bad2.to_c()
     assert lib.b200ba_test_pack(ctypes.byref(co), ctypes.byref(cp), 0, None, None, None, None, None, None,
                                 info.ctypes.data_as(ctypes.POINTER(ctypes.c_int64))) == -2
+
+
+def test_assembly_covariance_and_solve_errors_reach_b200ba_last_error():
+    # the problem assembly, the covariance estimate and the solve are separate translation units with one error string
+    lib = _bind_cov(_bind(load_library()))
+    lib.b200ba_assemble.argtypes = [ctypes.POINTER(_COptions), ctypes.POINTER(_CScene), ctypes.POINTER(_CConfig), ctypes.POINTER(ctypes.c_void_p)]
+    co, h = BundleAdjustmentOptions().to_c(), ctypes.c_void_p()
+    image_camera = np.array([1], np.int32)
+    sc = _CScene(num_images=1, image_camera=image_camera.ctypes.data_as(_i32p), num_cameras=1)
+    assert lib.b200ba_assemble(ctypes.byref(co), ctypes.byref(sc), ctypes.byref(_CConfig()), ctypes.byref(h)) == -2
+    assert lib.b200ba_last_error() == b"image references a camera outside the scene"
+    cov = _CCovOptions(7, 1e-8)
+    assert lib.b200ba_estimate_covariance(ctypes.byref(co), ctypes.byref(cov), ctypes.byref(_CProblem()), ctypes.byref(h)) == -2
+    assert lib.b200ba_last_error() == b"unknown covariance mode"
+    assert lib.b200ba_solve(None, None, None) == -1
+    assert lib.b200ba_last_error() == b"null argument"
+
 
 
 # ---------------------------------------------------------------- C++ problem assembly == the Python mirror's

@@ -32,7 +32,8 @@ from colmap_b200.synthetic import synthesize_ba_problem, synthesize_rig_problem
 from test_ba_cpu import _pack
 from test_ba_gpu import _assert_parity, _both, _gauge
 
-# ---------------------------------------------------------------- the thresholds of colmap_b200/csrc/bundle_adjustment.cu
+# ---------------------------------------------------------------- the thresholds of colmap_b200/csrc: ba_common.cuh (DENSE_MAX,
+# SPMV_SMEM_MAX, NARROW_MODELS) and bundle_adjustment.cu (the PCG step: PCG_FUSED_MAX, MID_STAGED_MAX, MID_SMEM_MAX)
 DENSE_MAX = 256                  # BA_DENSE_MAX: exact requests up to this nc factorise the reduced matrix densely
 PCG_FUSED_MAX = 65536            # BA_PCG_FUSED_MAX: single-CTA PCG vector step between SpMVs; above: five kernels
 MID_STAGED_MAX = 1024 * 5        # BA_PCG_T * BA_MID_EPT: ba_pcg_mid_staged_kernel
