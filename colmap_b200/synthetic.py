@@ -754,3 +754,71 @@ def make_sift_view_pair(n1, n2, overlap=0.5, noise=(0.0, 3.0), seed=0):
     inv = np.empty(n2, np.int64); inv[perm] = np.arange(n2)
     truth = np.stack([src, inv[np.arange(k)]], axis=1) if k else np.zeros((0, 2), np.int64)
     return FeatureDescriptorsToUnsignedByte(a), FeatureDescriptorsToUnsignedByte(b), truth
+
+
+def _project_two_view(model_id, params, X):
+    """ImgFromCam of the models make_guided_view_pair uses (sensor/models.h): SIMPLE_PINHOLE, SIMPLE_RADIAL,
+    SIMPLE_RADIAL_FISHEYE and EQUIRECTANGULAR; X is (n, 3) in the camera frame."""
+    p = np.asarray(params, np.float64)
+    if model_id == 17:
+        theta = np.arctan2(X[:, 0], X[:, 2])
+        phi = np.arcsin(np.clip(-X[:, 1] / np.linalg.norm(X, axis=1), -1, 1))
+        return np.stack([p[0] * (theta / (2 * np.pi) + 0.5), p[1] * (0.5 - phi / np.pi)], axis=1)
+    u, v = X[:, 0] / X[:, 2], X[:, 1] / X[:, 2]
+    if model_id == 8:
+        r = np.hypot(u, v)
+        s = np.where(r > 1e-12, np.arctan(r) / np.maximum(r, 1e-12), 1.0)
+        u, v = u * s, v * s
+    if model_id in (2, 8):
+        rad = p[3] * (u * u + v * v)
+        u, v = u + u * rad, v + v * rad
+    return np.stack([p[0] * u + p[1], p[0] * v + p[2]], axis=1)
+
+
+def make_guided_view_pair(n1, n2, model_id=0, plane=False, overlap=0.5, pixel_noise=0.5, seed=0):
+    """Two views of planted 3D points for guided matching.  Descriptors come from make_sift_view_pair (noisy copies of
+    a subset plus distractors); each planted copy (i1, i2) is a 3D point seen by both cameras, and its keypoints are
+    its projections with Gaussian pixel noise; every other keypoint is uniform over the image.  Both cameras share
+    `model_id`: 0 SIMPLE_PINHOLE, 2 SIMPLE_RADIAL, 8 SIMPLE_RADIAL_FISHEYE or 17 EQUIRECTANGULAR.  With `plane` the
+    points lie on one plane.  Returns a dict with desc1, desc2, xy1, xy2 ((n, 2) float32), camera1, camera2
+    (bundle_adjustment.Camera), truth, E (cam2_from_cam1: ray2^T E ray1 = 0), F (the pinhole F of E, for model 0),
+    H (the pixel homography of the plane, with `plane` and model 0)."""
+    from .bundle_adjustment import Camera
+    rng = np.random.default_rng(seed)
+    d1, d2, truth = make_sift_view_pair(n1, n2, overlap=overlap, seed=seed)
+    W, Hh = (1024, 512) if model_id == 17 else (640, 480)
+    params = {0: [500.0, 320.0, 240.0], 2: [500.0, 320.0, 240.0, -0.08], 8: [300.0, 320.0, 240.0, 0.03],
+              17: [float(W), float(Hh)]}[model_id]
+    cam = Camera(1, model_id, np.array(params, np.float64))
+    ang = rng.normal(0, 0.05, 3)
+    th = np.linalg.norm(ang)
+    k = ang / th
+    Kx = np.array([[0, -k[2], k[1]], [k[2], 0, -k[0]], [-k[1], k[0], 0]])
+    R = np.eye(3) + np.sin(th) * Kx + (1 - np.cos(th)) * Kx @ Kx
+    t = np.array([1.0, 0.1, 0.05]) + rng.normal(0, 0.05, 3)
+    tx = np.array([[0, -t[2], t[1]], [t[2], 0, -t[0]], [-t[1], t[0], 0]])
+    E = tx @ R
+    m = len(truth)
+    # points in front of both cameras, inside the pinhole field of view of camera 1
+    x = rng.uniform(-0.5, 0.5, (m, 2))
+    depth = np.full(m, 6.0) if plane else rng.uniform(4.0, 12.0, m)
+    X1 = np.concatenate([x * depth[:, None], depth[:, None]], axis=1)
+    if plane:   # the plane z = 6 tilted: n . X = d
+        nrm = np.array([0.1, -0.2, 1.0]); nrm /= np.linalg.norm(nrm)
+        dpl = 6.0
+        X1 = X1 * (dpl / (X1 @ nrm))[:, None]
+    X2 = X1 @ R.T + t
+    xy1 = rng.uniform([0, 0], [W, Hh], (n1, 2))
+    xy2 = rng.uniform([0, 0], [W, Hh], (n2, 2))
+    if m:
+        xy1[truth[:, 0]] = _project_two_view(model_id, params, X1) + rng.normal(0, pixel_noise, (m, 2))
+        xy2[truth[:, 1]] = _project_two_view(model_id, params, X2) + rng.normal(0, pixel_noise, (m, 2))
+    out = {"desc1": d1, "desc2": d2, "xy1": xy1.astype(np.float32), "xy2": xy2.astype(np.float32), "camera1": cam,
+           "camera2": Camera(2, model_id, np.array(params, np.float64)), "truth": truth, "E": E, "F": None, "H": None}
+    if model_id == 0:
+        K = np.array([[params[0], 0, params[1]], [0, params[0], params[2]], [0, 0, 1.0]])
+        Ki = np.linalg.inv(K)
+        out["F"] = Ki.T @ E @ Ki
+        if plane:
+            out["H"] = K @ (R + np.outer(t, nrm) / dpl) @ Ki
+    return out

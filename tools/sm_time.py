@@ -3,7 +3,10 @@ time, and Match end to end with both uploads), an exhaustive block of 50 images 
 MatchPairs, and the CPU oracle (tests/sm_oracle.c, a restatement of the rule, not the reference's code) on all host
 cores.  Prints the card's name and power limit beside the numbers, and one JSON line at the end.
 
-  python tools/sm_time.py [--reps 20] [--block 50] [--oracle-pairs 3]
+With --guided it times guided matching instead: one 8192 x 8192 pair per filter (E, F, H) with cross-check, the
+exhaustive block under F, and the guided CPU oracle (tests/sm_guided_oracle.c) on one E pair.
+
+  python tools/sm_time.py [--reps 20] [--block 50] [--oracle-pairs 3] [--guided]
 """
 import argparse
 import json
@@ -48,12 +51,17 @@ def main():
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--block", type=int, default=50)
     ap.add_argument("--oracle-pairs", type=int, default=3)
+    ap.add_argument("--guided", action="store_true")
     args = ap.parse_args()
     smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                          capture_output=True, text=True).stdout.strip()
     card = smi.splitlines()[0] if smi else "unknown"
     print("GPU:", card, flush=True)
     out = {"gpu": card}
+    if args.guided:
+        guided(args, out)
+        print(json.dumps(out))
+        return
 
     d1, d2, _ = make_sift_view_pair(N, N, seed=1)
     for cc in (True, False):
@@ -122,6 +130,66 @@ def main():
         print(f"CPU restatement of the rule (tests/sm_oracle.c, OpenMP, {os.cpu_count()} cores): {per:.2f} s per "
               f"8192 x 8192 pair with cross-check; GPU matches identical: {ok}", flush=True)
     print(json.dumps(out))
+
+
+def guided(args, out):
+    from colmap_b200.feature_matching import TwoViewGeometry
+    from colmap_b200.synthetic import make_guided_view_pair
+    s = make_guided_view_pair(N, N, model_id=0, plane=True, seed=1)
+    a = FeatureMatcherImage(1, s["desc1"], s["camera1"], s["xy1"])
+    b = FeatureMatcherImage(2, s["desc2"], s["camera2"], s["xy2"])
+    configs = {"E": TwoViewGeometry.CALIBRATED, "F": TwoViewGeometry.UNCALIBRATED, "H": TwoViewGeometry.PLANAR}
+    with CreateSiftFeatureMatcher(FeatureMatchingOptions(gpu_index="0")) as m:
+        for kind, config in configs.items():
+            g = TwoViewGeometry(config=config)
+            setattr(g, kind, s[kind])
+            for _ in range(3):
+                m.MatchGuided(4.0, a, b, g)
+            scan, total = [], []
+            for _ in range(args.reps):
+                m.MatchGuided(4.0, a, b, g)
+                sc, t = m.LastTiming()
+                scan.append(sc); total.append(t)
+            out["guided_" + kind] = {"matches": int(len(g.inlier_matches)), "scan_ms_min": stats(scan)[0],
+                                     "scan_ms_median": stats(scan)[1], "call_device_ms_median": stats(total)[1]}
+            print(f"guided {kind}, 8192 x 8192 with cross-check: {len(g.inlier_matches)} matches; guided scan "
+                  f"{stats(scan)[0]:.3f} ms min / {stats(scan)[1]:.3f} ms median, whole call on the device "
+                  f"{stats(total)[1]:.3f} ms (CUDA events, {args.reps} reps)", flush=True)
+
+    rng = np.random.default_rng(3)
+    images = [FeatureMatcherImage(im.image_id, im.descriptors, s["camera1"],
+                                  rng.uniform([0, 0], [640, 480], (N, 2)).astype(np.float32))
+              for im in block_images(args.block, N, seed=2)]
+    pairs = [(i, j) for i in range(len(images)) for j in range(i + 1, len(images))]
+    geos = [TwoViewGeometry(config=TwoViewGeometry.UNCALIBRATED, F=s["F"]) for _ in pairs]
+    with CreateSiftFeatureMatcher(FeatureMatchingOptions(gpu_index="0")) as m:
+        m.MatchGuidedPairs(images, pairs, geos, 4.0)
+        wall = []
+        for _ in range(3):
+            t0 = time.perf_counter()
+            res = m.MatchGuidedPairs(images, pairs, geos, 4.0)
+            wall.append(time.perf_counter() - t0)
+            sc, t = m.LastTiming()
+    nm = sum(len(r) for r in res)
+    out["guided_block_F"] = {"images": args.block, "pairs": len(pairs), "matches": int(nm), "call_s_min": min(wall),
+                             "pairs_per_s": len(pairs) / min(wall), "scan_ms": sc, "device_ms": t}
+    print(f"guided block {args.block} x {N} under F: {len(pairs)} pairs, {nm} matches; {len(pairs) / min(wall):.0f} "
+          f"pairs/s ({min(wall) * 1e3:.1f} ms per MatchGuidedPairs call, host clock; guided scans {sc:.1f} ms, device "
+          f"work {t:.1f} ms)", flush=True)
+
+    if args.oracle_pairs:
+        import oracle_smg
+        g1, g2 = oracle_smg.geo(s["camera1"], s["xy1"]), oracle_smg.geo(s["camera2"], s["xy2"])
+        t0 = time.perf_counter()
+        ref = oracle_smg.match(s["desc1"], s["desc2"], s["xy1"], s["xy2"], oracle_smg.E, s["E"], 4.0, g1, g2)
+        per = time.perf_counter() - t0
+        with CreateSiftFeatureMatcher(FeatureMatchingOptions(gpu_index="0")) as m:
+            g = TwoViewGeometry(config=TwoViewGeometry.CALIBRATED, E=s["E"])
+            m.MatchGuided(4.0, a, b, g)
+        ok = bool(np.array_equal(ref, g.inlier_matches))
+        out["guided_cpu_restatement"] = {"cores": os.cpu_count(), "s_per_pair_E": per, "equal_to_gpu": ok}
+        print(f"CPU restatement of the guided rule (tests/sm_guided_oracle.c, OpenMP, {os.cpu_count()} cores): "
+              f"{per:.2f} s per 8192 x 8192 E pair with cross-check; GPU matches identical: {ok}", flush=True)
 
 
 if __name__ == "__main__":
